@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native camera<-laser extrinsic solve.
+"""bench.py -- headline benchmark of the H100-native camera<-laser extrinsic solve.
 
 Workload (BASELINE.json configs[1]): 10^4 frames x 10^3 laser points per GPU, synthetic boards from the reference's
 simulation generator (main/calibr_simulation.cpp:10-108, exact-M mode, 1 cm range noise), identity initial guess.
@@ -12,7 +12,8 @@ One JSON line; everything the driver's parser keeps is nested under the contract
             heap array per frame) and times CamLaserCalibration(obs, Tcl, false) of the drop-in, entry to return -- gather/pack,
             PCIe, HBM layout, LM solve, analysis tail, tear-down; N ranks: rank 0 runs it on N devices of one process
   roofline  the fused sweep kernel alone: algorithmic bytes (24 B/residual + 40 B/frame + 224 B) / CUDA-event time per launch,
-            L2 flushed between launches, against the measured HBM copy bandwidth (MEASURED_PEAKS.json); nested: .planar (16 B per
+            L2 flushed between launches, against the measured HBM copy bandwidth (MEASURED_PEAKS.json when present, else the
+            H100 SXM data sheet's 3.35 TB/s); nested: .planar (16 B per
             residual, own denominator), .config3 (10^5 x 2000, 4.8 GB), .config5 (+ board-edge residuals, camera-chain poses)
   config    workload + .check (noise-free ground truth < 1e-9; collective evaluation = sum of the shards'), .strong_scaling
             (BASELINE configs[3], 2*10^9 residuals split over the N ranks), .step_device_ms (min / median / max of the K solves)
@@ -21,6 +22,10 @@ One JSON line; everything the driver's parser keeps is nested under the contract
 
 Multi-GPU (torchrun, one rank per GPU): weak scaling -- every rank holds 10^4 frames of a 10^4 x N frame problem; the 28
 normal-equation sums are exchanged inside the sweep kernel (NVLink peer stores) and every rank runs the identical LM update.
+
+--dump-outputs DIR (GPU arm): after the timed solves, rank 0 writes what the last timed solve returned to its caller --
+pose7.npy (T_cl as tx,ty,tz,qx,qy,qz,qw), summary.npy and trace.npy (float64, columns named in DUMP_*_FIELDS) -- so that
+two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -64,14 +69,33 @@ def parse_args():
     ap.add_argument("--no-config3", action="store_true", help="skip the supplementary 4.8 GB rows (configs[2] and configs[4])")
     ap.add_argument("--no-strong", action="store_true", help="skip the strong-scaling leg (configs[3], 48 GB over the N ranks)")
     ap.add_argument("--strong-frames", type=int, default=1_000_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed solve's outputs to DIR/<name>.npy (GPU arm)")
     return ap.parse_args()
+
+
+DUMP_SUMMARY_FIELDS = ("termination", "num_iterations", "num_successful_steps", "num_unsuccessful_steps", "num_sweeps",
+                       "initial_cost", "final_cost")
+DUMP_TRACE_FIELDS = ("iteration", "step_is_valid", "step_is_successful", "cost", "cost_change", "gradient_max_norm",
+                     "step_norm", "relative_decrease", "trust_region_radius")
+
+
+def dump_outputs(out_dir, x, summary, trace):
+    """What Problem.solve returned: the pose, the summary (device time left out: it is not an output of the math) and the
+    per-iteration trace, as float64 arrays."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "pose7.npy"), np.asarray(x, dtype=np.float64))
+    np.save(os.path.join(out_dir, "summary.npy"),
+            np.array([getattr(summary, k) for k in DUMP_SUMMARY_FIELDS], dtype=np.float64))
+    np.save(os.path.join(out_dir, "trace.npy"),
+            np.array([[getattr(it, k) for k in DUMP_TRACE_FIELDS] for it in trace], dtype=np.float64).reshape(-1, len(DUMP_TRACE_FIELDS)))
 
 
 def dist_env():
     return int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
 
 
-# ---- clocks during the timed region (B200_PROFILING.md) ----------------------------------------------------------
+# ---- clocks during the timed region ------------------------------------------------------------------------------
 class ClockSampler:
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
               "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -212,8 +236,6 @@ def run_reference(args):
         t_tot += dt
         ev_tot += ev
         steps_done += 1
-        if t_tot > 120.0:  # keep the whole run within a few minutes whatever --steps says
-            break
     value = ev_tot / t_tot
     sample = (f"each step = one full LM solve on the first {n} of {args.frames} frames x {args.beams} points "
               f"({n * args.beams} residuals, {iters} iterations); Ceres-shaped oracle port, evaluation on {cores} threads")
@@ -309,7 +331,7 @@ def run_ours(args):
     if args.gpus != world:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}: launch with torchrun --nproc-per-node {args.gpus}")
     torch.cuda.set_device(local_rank)
-    # clocks: 100 ms sampling period and nvidia-smi needs ~1 s to deliver its first line, the timed region lasts ~20 ms -- the
+    # clocks: 100 ms sampling period and nvidia-smi needs ~1 s to deliver its first line, the timed region is shorter -- the
     # sampler therefore runs from here (problem generation, communicator set-up, warm-up, timed solves, roofline legs)
     sampler = ClockSampler(local_rank)
     if rank == 0:
@@ -339,16 +361,10 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.SUM)
         return t.cpu().numpy()
 
-    peaks, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peaks, peak_src = 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peaks, peak_src = float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy burst)"
-    except Exception:
-        pass
-    traffic = {}
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            traffic = json.load(f)
     except Exception:
         pass
 
@@ -401,7 +417,7 @@ def run_ours(args):
     dev_ms, sweeps, iters, per_step = 0.0, 0, 0, []
     x = X0
     for _ in range(args.steps):
-        x, s, _ = prob.solve(X0, opt)
+        x, s, trace = prob.solve(X0, opt)
         dev_ms += s.device_ms
         per_step.append(s.device_ms)
         sweeps += s.num_sweeps
@@ -415,9 +431,11 @@ def run_ours(args):
     lm_iters_per_s = iters / (dev_ms * 1e-3)
     step_stats = {"min": float(np.min(per_step)), "median": float(np.median(per_step)), "max": float(np.max(per_step)),
                   "first": float(per_step[0]), "what": "device ms per solve on rank 0"}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, x, s, trace)
 
-    # ---- clocks: the timed region lasts ~20 ms, nvidia-smi samples every 100 ms and needs a second or so before its first line:
-    #      keep the device in exactly the timed region's state (the same solves, untimed) for ~2 s so that the sampler sees it ----
+    # ---- clocks: nvidia-smi samples every 100 ms and needs a second or so before its first line: keep the device in
+    #      exactly the timed region's state (the same solves, untimed) for a few seconds so that the sampler sees it ----
     for _ in range(2500):
         prob.solve(X0, opt)
     barrier()
@@ -448,8 +466,7 @@ def run_ours(args):
     # ---- roofline leg: the sweep kernel alone, L2 flushed between launches (local shard, no collective) ----
     roofline = kernel_row(prob, x, args.kernel_launches, peaks, "clc_sweep_kernel<LOSS,LM> general, 24 B/residual")
     k_b2b = prob.bench_eval(x, args.kernel_launches, flush_l2=False)
-    roofline.update({"traffic": traffic.get("dram_bytes_per_launch"), "traffic_source": traffic.get("source"),
-                     "peak_source": peak_src,
+    roofline.update({"peak_source": peak_src,
                      "l2": "flushed between launches (256 MiB written, then read back: no dirty lines left)",
                      "back_to_back_no_flush_ms": float(np.mean(k_b2b))})
 
@@ -457,14 +474,13 @@ def run_ours(args):
     prob.set_planar_mode(1)
     if prob.planar:
         row = kernel_row(prob, x, args.kernel_launches, peaks, "clc_sweep_kernel<LOSS,LM,PLANAR>, 16 B/residual (own denominator)")
-        row["traffic"] = (traffic.get("planar") or {}).get("dram_bytes_per_launch")
         row["speedup_over_24B_kernel"] = roofline["kernel_ms_mean"] / row["kernel_ms_mean"]
         _, srow = solve_row(prob, opt, args.steps, total_points, max_over_ranks, barrier)
         row["full_lm_solve"] = srow
         roofline["planar"] = row
     # the sampler ran from process start over the warm-up, the timed solves and the roofline legs (nvidia-smi needs a second or
-    # two before its first line, the timed solves last 20 ms); it stops here: the 48 GB strong-scaling leg below runs into
-    # the software power cap and is not what `value` / `roofline` were measured under
+    # two before its first line); it stops here: the 48 GB strong-scaling leg below is not what `value` / `roofline` were
+    # measured under
     clocks = sampler.stop() if rank == 0 else None
 
     # ---- strong scaling: BASELINE configs[3] (10^6 frames x 2*10^3 points = 2*10^9 residuals, 48 GB) over the N ranks ----
@@ -499,7 +515,7 @@ def run_ours(args):
                "h2d_bytes_per_step": int(dj["h2d_bytes_per_call"]), "d2h_bytes_per_step": int(dj["d2h_bytes_per_call"]),
                "ms_per_step": dj["body_ms_median"], "ms_per_step_mean": dj["body_ms_mean"], "ms_per_step_min": dj["body_ms_min"],
                "ms_per_step_max": dj["body_ms_max"], "steps": e2e_steps,
-               "statistic": "median over the steps (the host side shares a 16-CPU container quota with the launcher; single "
+               "statistic": "median over the steps (the host side shares the container's CPU quota with the launcher; single "
                             "steps that hit a scheduler stall are visible in ms_per_step_max / _mean)",
                "what": "C++ drop-in, pageable std::vector<Oberserve> input: CamLaserCalibration() entry to return",
                "phases_ms": dj["phases_ms_median"], "raw_h2d_ms_same_bytes": dj["raw_h2d_ms_same_bytes"],
@@ -528,8 +544,6 @@ def run_ours(args):
             big.set_planar_mode(1)
             r3p = kernel_row(big, x, 20, peaks, "planar, 16 B/residual")
             _, r3p["full_lm_solve"] = solve_row(big, opt, 2, 2e8, max_over_ranks, barrier)
-            r3["traffic"] = (traffic.get("config3") or {}).get("dram_bytes_per_launch")
-            r3p["traffic"] = ((traffic.get("config3") or {}).get("planar") or {}).get("dram_bytes_per_launch")
             r3["planar"] = r3p
             r3["workload"] = "BASELINE configs[2]: 100000 frames x 2000 points (4.8 GB)"
             roofline["config3"] = r3
@@ -541,7 +555,6 @@ def run_ours(args):
             r5["gt_rot_err_rad"], r5["gt_trans_err_m"] = pose_error_vs_ground_truth(x5)
             c5.set_planar_mode(1)
             r5p = kernel_row(c5, x, 20, peaks, "planar + edge tail, 16 B/residual + 56 B/edge residual")
-            r5["traffic"] = (traffic.get("config5") or {}).get("dram_bytes_per_launch")
             r5["planar"] = r5p
             r5["workload"] = ("BASELINE configs[4]: 100000 frames x 2000 points + 200000 board-edge residuals, board poses from "
                               "the equidistant (Kannala-Brandt) camera chain with 0.3 px corner noise")
@@ -558,7 +571,7 @@ def run_ours(args):
         cfg.update({"sharding": (f"frames by rank, {world} ranks, 28-double all-reduce per sweep: " +
                                  ("ncclAllReduce between kernels" if args.nccl_allreduce else
                                   "fused into the sweep kernel (NVLink peer stores, rank-order sum)")) if world > 1 else "single GPU",
-                    "l2": f"inputs ({roofline['algorithmic_bytes_per_launch'] / 1e6:.0f} MB/GPU) > 126 MB L2; roofline leg also flushes L2 between launches",
+                    "l2": f"inputs ({roofline['algorithmic_bytes_per_launch'] / 1e6:.0f} MB/GPU) > 50 MB L2; roofline leg also flushes L2 between launches",
                     "lm": "one fused residual+Jacobian+reduce sweep per LM iteration",
                     "kernels": "general three-stream kernels (24 B/residual contract row); planar rows separate",
                     "check": check, "strong_scaling": strong, "step_device_ms": step_stats})

@@ -1,4 +1,4 @@
-"""Compiles libclc_b200.so (sm_100a only) in-tree with nvcc.  No GPU is needed to build."""
+"""Compiles libclc_b200.so (sm_90a only) in-tree with nvcc.  No GPU is needed to build."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(PKG_DIR, "libclc_b200.so")
 SOURCES = ["clc_api.cu", "clc_pack.cpp"]
 HEADERS = ["clc_kernels.cuh", "clc_math.cuh", "clc_lm.cuh", "clc_expand.cuh", "clc_linefit.cuh", "clc_camera.cuh", "clc_upload.inl"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
     "-diag-suppress", "177",
@@ -56,18 +56,10 @@ REPO = os.path.dirname(PKG_DIR)
 DROPIN_SRC = os.path.join(PKG_DIR, "host", "LaseCamCalB200.cpp")
 BENCH_SRC = os.path.join(PKG_DIR, "host", "dropin_bench.cpp")
 BENCH_EXE = os.path.join(PKG_DIR, "host", "clc_dropin_bench")
-REFERENCE_INCLUDE = "/root/reference/include"
-
-
 def interface_include_dirs():
-    """Include path of the reference interface: the reference's own include/LaseCamCalCeres.h when the tree is present
-    (build container), else the test stand-in; Eigen itself is not in this image, so its few types come from tests/stubs."""
-    dirs = []
-    if os.path.exists(os.path.join(REFERENCE_INCLUDE, "LaseCamCalCeres.h")):
-        dirs.append(REFERENCE_INCLUDE)
-    dirs.append(os.path.join(REPO, "tests", "stubs"))
-    dirs.append(os.path.join(REPO, "include"))
-    return dirs
+    """Include path of the reference interface: the stand-in of LaseCamCalCeres.h and the few Eigen types it needs
+    (tests/stubs), then the C ABI.  A real integration puts the reference's own include/ first (INTEGRATION.md)."""
+    return [os.path.join(REPO, "tests", "stubs"), os.path.join(REPO, "include")]
 
 
 def cxx_command(sources, out, extra=()):

@@ -1,6 +1,6 @@
 // clc_api.cu -- host side of libclc_b200.so: the C ABI declared in include/clc_b200.h.
 //
-// No CPU fallback lives here: every entry point drives the sm_100a kernels of clc_kernels.cuh and fails loudly
+// No CPU fallback lives here: every entry point drives the sm_90a kernels of clc_kernels.cuh and fails loudly
 // (status code + clc_last_error()) when CUDA is unusable.  The only host arithmetic is O(1) dense work on the
 // reduced 6x6 / 9x9 systems for the two diagnostic outputs the reference prints (singular values, closed form).
 #include <cuda_runtime.h>
@@ -382,8 +382,7 @@ int allreduce_sums(clc_problem* p, int count) {
 }
 
 // Waits for a stream with a short spin before blocking: a blocking cudaStreamSynchronize puts the thread to sleep and the wake-up
-// costs tens of microseconds (measured: 40-90 us per mid-solve poll inside a CPU-quota'd container, profiles/r2_loop_modes2.txt),
-// which is as long as a whole sweep at BASELINE configs[1].  Work that takes longer than the spin budget falls back to blocking.
+// costs tens of microseconds (more inside a CPU-quota'd container), which is as long as a whole sweep at BASELINE configs[1].  Work that takes longer than the spin budget falls back to blocking.
 cudaError_t sync_stream_low_latency(cudaStream_t st) {
   const auto t0 = std::chrono::steady_clock::now();
   for (;;) {
@@ -425,7 +424,7 @@ int partition(clc_problem* p) {
     if (blocks_needed < p->grid) p->grid = (int)blocks_needed;
     // the reference's own sizes (50 boards x 180 beams, reference main/calibr_simulation.cpp:34,79) fit ONE block: a
     // single-block grid lets the kernel run the whole LM loop by itself (no launch, no inter-block exchange per iteration)
-    int64_t single_block_max = (int64_t)clc::kWarps * 8 * clc::kChunk;  // up to 8 stages per warp and sweep (16384 points)
+    int64_t single_block_max = (int64_t)clc::kWarps * 8 * clc::kChunk;  // up to 8 stages per warp and sweep (12288 points)
     if (const char* env = std::getenv("CLC_SINGLE_BLOCK_MAX_POINTS")) single_block_max = std::atoll(env);
     if (p->n_points <= single_block_max) p->grid = 1;
   }
@@ -542,7 +541,7 @@ int init_device(clc_problem* p, int device) {
   p->device = device;
   CLC_CUDA(cudaSetDevice(device));
   // per-device facts are queried once (cudaGetDeviceProperties alone costs about a millisecond, which would dominate
-  // the reference-sized calls: 50 frames x 180 points solve in 0.25 ms)
+  // the reference-sized calls: 50 frames x 180 points solve in a fraction of a millisecond)
   struct DeviceInfo { bool valid = false; int major = 0, minor = 0, sms = 0; };
   static std::mutex info_mutex;
   static DeviceInfo info[64];
@@ -564,17 +563,16 @@ int init_device(clc_problem* p, int device) {
     std::lock_guard<std::mutex> lock(info_mutex);
     if (device < 64) info[device] = di;
   }
-  if (di.major < 10)
-    return fail(CLC_ERR_CUDA, std::string("libclc_b200 is built for sm_100a only; device is sm_") + std::to_string(di.major) +
+  if (di.major != 9 || di.minor != 0)
+    return fail(CLC_ERR_CUDA, std::string("libclc_b200 is built for sm_90a only; device is sm_") + std::to_string(di.major) +
                                   std::to_string(di.minor));
   p->num_sms = di.sms;
   CLC_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   return CLC_OK;
 }
 
-// Placement of the coordinate arrays relative to each other.  Measured at BASELINE configs[2] (profiles/r2_layout_ab.txt):
-// the sweep kernel streams fastest when x, y and z start at the same offset within a 2 MiB page, so that a warp's three
-// bulk copies of one stage cross page boundaries together; any other relative shift that was tried costs 3-8 %.  x and y
+// Placement of the coordinate arrays relative to each other: x, y and z start at the same offset within a 2 MiB page, so
+// that a warp's three bulk copies of one stage cross page boundaries together.  x and y
 // live in one allocation, y starting skew_y bytes after the end of x (default: up to the next address congruent to x mod
 // 2 MiB; small problems are packed); z is its own allocation (it exists only for non-planar data) whose start is shifted so
 // that (z - x) mod 2 MiB == skew_z (default 0).  CLC_SKEW_Y / CLC_SKEW_Z (bytes) override both: the experiment knobs.
@@ -1157,7 +1155,7 @@ struct SolveCtx {
 };
 
 // L2 residency across LM iterations: every iteration re-reads the same coordinate arrays.  When they are not much larger than
-// the 126 MB L2, a persisting access-policy window over the x,y block keeps a hash-selected share of their lines (hitRatio =
+// the 50 MB L2, a persisting access-policy window over the x,y block keeps a hash-selected share of their lines (hitRatio =
 // set-aside / window) resident from one sweep to the next, so that share is not fetched from HBM again.  The set-aside is a
 // device-wide limit: it is raised on first use and left in place.  Only the solve loop runs under the window; the measurement
 // hook clc_bench_eval (L2 flushed between launches: the 24 B / 16 B roofline rows) does not.
@@ -1315,7 +1313,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
   while (launched < max_sweeps) {
     // the first batch is twice as long: a solve from the identity or from the closed form takes 6-16 sweeps (reference sizes and
     // BASELINE configs alike), and every host poll in the middle of a solve stalls the device for longer than the two or three
-    // no-op sweeps a too-long batch costs (3 us each; profiles/r2_loop_modes2.txt)
+    // no-op sweeps a too-long batch costs (a few microseconds each)
     const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
     // iteration-major order: sweep i of every shard is queued before sweep i+1 of any, so no device's queue can fill up
     // with kernels that wait for a peer whose launches have not been issued yet
@@ -1414,9 +1412,10 @@ int clc_line_fit_points(const double* points_xyz, int64_t n, double line[2], int
   int device = 0;
   CLC_CUDA(cudaGetDevice(&device));
   if (c.device != device) {
-    int major = 0;
+    int major = 0, minor = 0;
     CLC_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
-    if (major < 10) return fail(CLC_ERR_CUDA, "libclc_b200 is built for sm_100a only");
+    CLC_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (major != 9 || minor != 0) return fail(CLC_ERR_CUDA, "libclc_b200 is built for sm_90a only");
     if (c.stream) { cudaStreamDestroy(c.stream); c.stream = nullptr; }
     if (c.d_pts) { cudaFree(c.d_pts); c.d_pts = nullptr; c.capacity = 0; }
     CLC_CUDA(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
@@ -2033,7 +2032,7 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   if (flush_l2 && !p->flush_buf) {
-    p->flush_n = ((int64_t)256 << 20) / sizeof(double);  // 256 MiB > 126 MB of L2
+    p->flush_n = ((int64_t)256 << 20) / sizeof(double);  // 256 MiB > 50 MB of L2
     CLC_CUDA(cudaMallocAsync(&p->flush_buf, sizeof(double) * p->flush_n, p->stream));
   }
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));

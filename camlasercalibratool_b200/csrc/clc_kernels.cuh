@@ -1,4 +1,4 @@
-// clc_kernels.cuh -- the sm_100a kernels.
+// clc_kernels.cuh -- the sm_90a kernels.
 //
 // K1  clc_sweep_kernel   fused residual + Jacobian + Cauchy weight + reduce over every laser point
 //                        (HBM-bandwidth bound FP64 map-reduce; 24 B per residual streamed with 128-bit loads)
@@ -15,11 +15,12 @@
 
 namespace clc {
 
-// Launch shape chosen from a measured sweep of {128..512 threads} x {1..4 blocks/SM} x {1..6 stages} x {64,128,256}-point
-// stages on B200 (profiles/r1_variant_sweep.txt): one 16-warp block per SM with 2 stages per warp is the fastest at both
-// 240 MB and 4.8 GB; deeper rings let the warps favoured by the issue arbiter run ahead and lengthen the tail.
+// Launch shape: one 12-warp block per SM with 2 stages per warp.  On an H100 (sm_90a) 384 threads leave the streaming
+// instantiations 168 registers and no spills; with 512 threads (128 registers) they spill ~0.5 KB per thread and run ~17 %
+// slower at configs[1] and ~10 % at configs[2] (320 threads ties with 384, 448 is as slow as 512; a third stage or two
+// 256-thread blocks per SM gain nothing).  Dynamic shared memory per block: ~111 KiB general, ~135 KiB planar.
 #ifndef CLC_THREADS
-#define CLC_THREADS 512
+#define CLC_THREADS 384
 #endif
 #ifndef CLC_BLOCKS_PER_SM
 #define CLC_BLOCKS_PER_SM 1
@@ -46,7 +47,7 @@ constexpr int kMailboxSlot = 64;      // doubles per (parity, source rank) mailb
 #ifndef CLC_PLANAR_CHUNK
 #define CLC_PLANAR_CHUNK (CLC_CHUNK * 2)
 #endif
-// the two-stream (planar, z == 0) kernels: 2 KiB bulk copies (measured: 256-point stages stream 10 % faster than 128/192)
+// the two-stream (planar, z == 0) kernels: 256-point stages, one 2 KiB bulk copy per coordinate array
 constexpr int kPlanarStages = CLC_PLANAR_STAGES;
 constexpr int kPlanarChunk = CLC_PLANAR_CHUNK;
 static_assert(kChunk % 64 == 0 && kPlanarChunk % 64 == 0, "stages are made of 64-point groups");
@@ -353,8 +354,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     if (lane == 0) {
       const int c = LOOP ? next_c : issued, st = issued % NST;
       double* dst = ring + st * SST;
-      // always a whole stage (the arrays are zero padded beyond the last point; the ranges are whole stages): measured, a
-      // short last stage in 64-point units costs more than the idle warps it saves (profiles/r2_variant_sweep.txt)
+      // always a whole stage (the arrays are zero padded beyond the last point; the ranges are whole stages)
       const int64_t src = p0 + (int64_t)c * CH;  // multiple of the stage size -> 1 KiB aligned
       if (slot_was_read) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_expect_tx(bars + st, (PLANAR ? 2 : 3) * CH * 8);
@@ -449,7 +449,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
   {
     double pose[7];
 #pragma unroll
-    // plain (L1-cached) loads: 2368 warps read the same 56 bytes -- one L2 request per SM instead of one per warp (L1 is
+    // plain (L1-cached) loads: every warp of the grid reads the same 56 bytes -- one L2 request per SM instead of one per warp (L1 is
     // invalidated at every kernel launch, so the pose written by the previous sweep's block 0 is what arrives)
     for (int i = 0; i < 7; ++i) pose[i] = (LOOP && sw > 0) ? s_next[i] : args.pose7[i];
     make_pose_consts(pose, &pc);
@@ -970,7 +970,7 @@ __global__ void clc_gen_points_kernel(uint64_t seed, double sigma, int64_t frame
 }
 
 // L2 flush for the measurement hook: overwrite a buffer larger than L2, then read it back.  The read pass matters:
-// after the write pass L2 is full of DIRTY lines whose write-back (~126 MB of DRAM writes) would otherwise be charged
+// after the write pass L2 is full of DIRTY lines whose write-back (~50 MB of DRAM writes) would otherwise be charged
 // to the kernel being timed; after the read pass L2 holds clean, unrelated lines.
 __global__ void clc_flush_kernel(double* buf, int64_t n, double v) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)

@@ -1,9 +1,9 @@
 // clc_small.cuh -- the whole Levenberg-Marquardt solve of a SMALL problem in one launch of one thread-block cluster.
 //
-// The reference's own problems are tiny for a B200: 50 board poses x <= 180 laser points (reference
+// The reference's own problems are tiny for an H100: 50 board poses x <= 180 laser points (reference
 // main/calibr_simulation.cpp:34,79), a few thousand residuals.  The streaming sweep kernel (clc_kernels.cuh) is built for
-// 10^7..10^9 points -- per-warp TMA rings, moment expansion, a 148-block gather -- and at this size spends its time in
-// machinery: 18 us per LM iteration even when it loops inside one launch (profiles/r2_variant_sweep.txt).  Here instead
+// 10^7..10^9 points -- per-warp TMA rings, moment expansion, a one-block-per-SM gather -- and at this size spends its time
+// in machinery even when it loops inside one launch.  Here instead
 //   * one cluster of 8 CTAs x 256 threads; every thread loads its <= 8 residuals (point, frame index, 1/#points of the frame)
 //     ONCE into registers and keeps them for the whole solve;
 //   * per LM iteration every thread evaluates its residuals against the current pose and accumulates the 28 sums (21 of H,

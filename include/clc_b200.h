@@ -1,5 +1,5 @@
 /*
- * clc_b200.h -- C ABI of libclc_b200.so: the B200-native (sm_100a) implementation of the camera<-laser
+ * clc_b200.h -- C ABI of libclc_b200.so: the H100-native (sm_90a) implementation of the camera<-laser
  * extrinsic solve of MegviiRobot/CamLaserCalibraTool.
  *
  * The reference has no FFI: its "operator API" for this path is four C++ free functions plus one struct
@@ -8,7 +8,7 @@
  * replacement (same signatures, same Oberserve struct) and INTEGRATION.md shows the CMake change.
  *
  * Plain C, POD only, int status codes (0 = CLC_OK), no exceptions cross the boundary, no torch types.
- * There is NO CPU fallback: every entry point fails with CLC_ERR_CUDA if no sm_100 device is usable.
+ * There is NO CPU fallback: every entry point fails with CLC_ERR_CUDA if no sm_90 device is usable.
  *
  * Data conventions (identical to the marshalled form of std::vector<Oberserve>):
  *   frame_pose[f*7 .. +7] = qx,qy,qz,qw (Eigen coeff order of Oberserve::tagPose_Qca), tx,ty,tz (tagPose_tca)
@@ -295,7 +295,7 @@ int clc_problem_streamed_bytes(const clc_problem* p, int64_t* bytes);
  * drops the z stream from HBM and runs two-stream kernels whose results equal the general ones (up to summation order) on such
  * data (SURVEY.md 8(d): a separate roofline row, 16 B per residual).  mode 1 = automatic (default), 0 = always the
  * general three-stream kernels (an all-zero z stream is re-materialised if it was dropped).  Problems too small to give
- * every warp of the grid a 256-point stage (about 6*10^5 points on a B200) are latency-bound and stay on the general
+ * every warp of the grid a 256-point stage (about 4*10^5 points on an H100) are latency-bound and stay on the general
  * kernels in either mode (environment override for tests: CLC_PLANAR_MIN_POINTS). */
 int clc_problem_set_planar_mode(clc_problem* p, int mode);
 /* Statistics of this process's most recent host -> HBM point upload: wall time of the pipeline, time the issuing thread

@@ -2,7 +2,7 @@
 
 * `-m "not gpu"` : oracle vs numpy twin vs golden fixtures, host logic of the product (compiled with g++ from the
                    same CLC_HD sources the GPU runs), ABI surface of libclc_b200.so, world_size-2 gloo sharding.
-* `-m gpu`       : parity of the CUDA path (through the C ABI) against the oracle on a B200.
+* `-m gpu`       : parity of the CUDA path (through the C ABI) against the oracle on an H100.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu on the GPU box")
 
 
 def _has_gpu() -> bool:

@@ -15,19 +15,16 @@ def build_driver(out_dir):
 
     _lib.load()
     exe = os.path.join(out_dir, "host_dropin_test")
-    # against the reference's own include/LaseCamCalCeres.h when /root/reference exists (build container), else the stand-in
     subprocess.check_call(_build.cxx_command([os.path.join(ROOT, "tests", "host_dropin_test.cpp"), _build.DROPIN_SRC], exe))
     return exe
 
 
-def test_dropin_compiles_against_the_reference_header_when_present():
+def test_dropin_compiles_against_the_interface_stand_in():
     from camlasercalibratool_b200 import _build
 
     dirs = _build.interface_include_dirs()
-    if os.path.exists("/root/reference/include/LaseCamCalCeres.h"):
-        assert dirs[0] == "/root/reference/include"  # the genuine interface wins over tests/stubs/LaseCamCalCeres.h
-    else:
-        assert dirs[0].endswith(os.path.join("tests", "stubs"))
+    assert dirs[0] == os.path.join(ROOT, "tests", "stubs")  # nothing outside the repository is on the include path
+    assert all(os.path.realpath(d).startswith(os.path.realpath(ROOT) + os.sep) for d in dirs)
 
 
 def test_bench_driver_builds():
