@@ -19,6 +19,7 @@
 
 #include "../../include/clc_b200.h"
 #include "clc_kernels.cuh"
+#include "clc_l2_plan.h"
 #include "clc_linefit.cuh"
 #include "clc_small.cuh"
 
@@ -234,6 +235,7 @@ struct clc_problem {
   int device = 0;
   cudaStream_t stream = nullptr;
   int num_sms = 0;
+  int64_t l2_bytes = 0;  // the device's L2 size
   int grid = 0;
   int64_t n_frames = 0, n_points = 0, n_points_padded = 0, n_edges = 0;
   int use_loss = 1;
@@ -260,6 +262,8 @@ struct clc_problem {
   bool use_pdl = true;                   // CLC_PDL=0 disables programmatic dependent launch in the LM loop
   int64_t l2_persist_bytes = 0;          // persisting-L2 window over the coordinate arrays during LM solves (0 = off)
   bool l2_window_set = false;
+  int64_t l2_resident_bytes = -1;        // CLC_L2_RESIDENT_MB: L2 budget of the resident stages (-1 = the default share of L2)
+  int resident_chunks = 0;               // stages per warp kept in L2 during LM solves (clc_l2_plan.h; set by partition)
   bool small_kernel = true;              // CLC_SMALL_KERNEL=0: never use the one-cluster kernel of clc_small.cuh
   int loop_in_kernel = 1;                // CLC_LOOP_IN_KERNEL: 0 one launch per LM iteration; 1 single-block problems run the whole
                                          // LM loop in one launch; 2 every problem does (persistent grid, block 0 hands out the poses)
@@ -300,6 +304,7 @@ clc::ProblemView make_view(const clc_problem* p) {
   v.n_points = p->n_points;
   v.n_edges = p->n_edges;
   v.per_warp = p->per_warp;
+  v.resident_chunks = p->resident_chunks;
   v.a2 = p->cauchy_a * p->cauchy_a;
   v.inv_a2 = 1.0 / v.a2;
   return v;
@@ -313,7 +318,7 @@ int set_device(const clc_problem* p) {
 // one K1 launch on the problem's stream
 // collective: the sums of this launch are to be all-reduced (in-kernel when the peer path is active)
 int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* d_pose, const int* d_done,
-                 clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1) {
+                 clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false) {
   clc::SweepArgs a;
   a.pose7 = d_pose;
   a.done = d_done;
@@ -324,6 +329,7 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   a.lm = d_lm;
   a.use_loss = loss ? 1 : 0;
   a.use_edges = edges ? 1 : 0;
+  a.l2_hints = l2_hints ? 1 : 0;
   a.loop_sweeps = loop_sweeps;
   a.timing = p->timing;
   a.nranks = 1;
@@ -437,6 +443,13 @@ int partition(clc_problem* p) {
   CLC_CUDA(cudaMallocAsync(&p->warp_first_frame, sizeof(int) * n_warps, p->stream));
   const size_t ll_bytes = sizeof(unsigned long long) * 2 * (size_t)p->grid * clc::kMaxOut;
   CLC_CUDA(cudaMallocAsync(&p->partials_ll, ll_bytes, p->stream));
+  {
+    // L2 residency of LM solves (clc_l2_plan.h); the persisting-L2 window, when it is configured, takes its place
+    const int64_t stage_bytes = (int64_t)(p->planar ? 2 : 3) * chunk * 8;
+    const bool latency_bound = p->n_points <= clc::kSmallMaxResiduals;  // the one-cluster kernel's problems
+    const int64_t budget = p->l2_persist_bytes > 0 ? 0 : clc::l2_resident_budget(p->l2_bytes, p->l2_resident_bytes);
+    p->resident_chunks = clc::l2_resident_chunks(budget, p->grid, clc::kWarps, p->per_warp / chunk, stage_bytes, latency_bound);
+  }
   CLC_CUDA(cudaMemsetAsync(p->partials_ll, 0, ll_bytes, p->stream));  // tag 0 never matches a launch (sequence numbers start at 1)
   const int threads = 256;
   const int blocks = (int)((n_warps + threads - 1) / threads);
@@ -491,6 +504,7 @@ int finish_create(clc_problem* p) {
   if (const char* env = std::getenv("CLC_LOOP_IN_KERNEL")) p->loop_in_kernel = std::atoi(env);
   if (const char* env = std::getenv("CLC_SMALL_KERNEL")) p->small_kernel = std::atoi(env) != 0;
   if (const char* env = std::getenv("CLC_L2_PERSIST_MB")) p->l2_persist_bytes = (int64_t)std::atoll(env) << 20;
+  if (const char* env = std::getenv("CLC_L2_RESIDENT_MB")) p->l2_resident_bytes = std::max<int64_t>(0, (int64_t)std::atoll(env) << 20);
   CLC_CUDA(cudaMallocAsync(&p->sums, sizeof(double) * clc::kMaxOut, p->stream));
   CLC_CUDA(cudaMallocAsync(&p->pose, sizeof(double) * 8, p->stream));
   CLC_CUDA(cudaMallocAsync(&p->launch_seq, sizeof(unsigned int), p->stream));
@@ -542,7 +556,7 @@ int init_device(clc_problem* p, int device) {
   CLC_CUDA(cudaSetDevice(device));
   // per-device facts are queried once (cudaGetDeviceProperties alone costs about a millisecond, which would dominate
   // the reference-sized calls: 50 frames x 180 points solve in a fraction of a millisecond)
-  struct DeviceInfo { bool valid = false; int major = 0, minor = 0, sms = 0; };
+  struct DeviceInfo { bool valid = false; int major = 0, minor = 0, sms = 0, l2 = 0; };
   static std::mutex info_mutex;
   static DeviceInfo info[64];
   DeviceInfo di;
@@ -554,6 +568,7 @@ int init_device(clc_problem* p, int device) {
     CLC_CUDA(cudaDeviceGetAttribute(&di.major, cudaDevAttrComputeCapabilityMajor, device));
     CLC_CUDA(cudaDeviceGetAttribute(&di.minor, cudaDevAttrComputeCapabilityMinor, device));
     CLC_CUDA(cudaDeviceGetAttribute(&di.sms, cudaDevAttrMultiProcessorCount, device));
+    CLC_CUDA(cudaDeviceGetAttribute(&di.l2, cudaDevAttrL2CacheSize, device));
     // keep freed device memory in the pool instead of returning it to the driver at every synchronisation
     cudaMemPool_t pool;
     CLC_CUDA(cudaDeviceGetDefaultMemPool(&pool, device));
@@ -567,6 +582,7 @@ int init_device(clc_problem* p, int device) {
     return fail(CLC_ERR_CUDA, std::string("libclc_b200 is built for sm_90a only; device is sm_") + std::to_string(di.major) +
                                   std::to_string(di.minor));
   p->num_sms = di.sms;
+  p->l2_bytes = di.l2;
   CLC_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
   return CLC_OK;
 }
@@ -1217,7 +1233,8 @@ int solve_launch_one(clc_problem* p, SolveCtx* ctx, int loop_sweeps = 1) {
   // fused mode: one kernel per LM iteration, chained with programmatic dependent launch (the next sweep prefetches
   // its first stages while this one's block 0 reduces and updates)
   rc = launch_sweep(p, clc::kModeLM, ctx->loss, ctx->edges, p->lm->core.cand, &p->lm->core.done,
-                    ctx->fused_update ? p->lm : nullptr, /*collective=*/true, /*pdl=*/ctx->fused_update && p->use_pdl, loop_sweeps);
+                    ctx->fused_update ? p->lm : nullptr, /*collective=*/true, /*pdl=*/ctx->fused_update && p->use_pdl, loop_sweeps,
+                    /*l2_hints=*/true);
   if (rc != CLC_OK) return rc;
   if (!ctx->fused_update) {
     rc = allreduce_sums(p, clc::kNumSums);
@@ -1236,8 +1253,22 @@ int solve_poll_enqueue(clc_problem* p) {
   return CLC_OK;
 }
 
-int solve_finish(clc_problem* p, double pose7[7], clc_lm_summary* summary, clc_lm_iteration* trace, int trace_cap) {
+// end of a solve: the lines its sweeps kept with evict_last go back to the normal eviction priority (clc_l2_demote_kernel)
+int l2_demote(clc_problem* p) {
+  if (p->resident_chunks == 0) return CLC_OK;
   int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  const int chunk = p->planar ? clc::kPlanarChunk : clc::kChunk;
+  const int64_t n_warps = (int64_t)p->grid * clc::kWarps;
+  const int64_t lines = n_warps * p->resident_chunks * (chunk / 16);
+  const int threads = 256;
+  clc::clc_l2_demote_kernel<<<(unsigned)((lines + threads - 1) / threads), threads, 0, p->stream>>>(make_view(p), n_warps, chunk);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+int solve_finish(clc_problem* p, double pose7[7], clc_lm_summary* summary, clc_lm_iteration* trace, int trace_cap) {
+  int rc = l2_demote(p);  // part of the solve: before ev1
   if (rc != CLC_OK) return rc;
   CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
   rc = l2_window(p, false);
@@ -1281,6 +1312,16 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
   int rc = CLC_OK;
   for (int g = 0; g < n && rc == CLC_OK; ++g) rc = solve_begin(ps[g], pose7, opt, &ctx[g]);
   if (rc != CLC_OK) return rc;
+  // an abandoned solve (an error below) still demotes the L2 lines its sweeps kept resident; solve_finish does it otherwise
+  struct DemoteOnExit {
+    clc_problem* const* ps;
+    int n;
+    bool armed;
+    ~DemoteOnExit() {
+      if (armed)
+        for (int g = 0; g < n; ++g) l2_demote(ps[g]);
+    }
+  } demote_on_exit{ps, n, true};
   const int max_sweeps = ctx[0].max_sweeps;
   int launched = 0;
   // Small problems (the reference's own sizes): the whole solve in one launch of one thread-block cluster that keeps every
@@ -1336,6 +1377,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
     }
     if (all_done) break;
   }
+  demote_on_exit.armed = false;
   double ms_max = 0.0;
   int first_rc = CLC_OK;
   for (int g = n - 1; g >= 0; --g) {  // shard 0 last: its pose / summary / trace are the ones returned (all shards agree)

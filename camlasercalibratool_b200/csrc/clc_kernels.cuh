@@ -84,6 +84,7 @@ struct ProblemView {
   int64_t n_points;
   int64_t n_edges;            // 2 * n_frames or 0
   int64_t per_warp;           // points per warp (multiple of the kernel family's stage size)
+  int resident_chunks;        // LM solves: the last resident_chunks stages of every warp's range are kept in L2 (clc_l2_plan.h)
   double inv_a2;              // 1 / cauchy_a^2
   double a2;                  // cauchy_a^2
 };
@@ -98,6 +99,7 @@ struct SweepArgs {
   LmState* lm;                // non-null: the last block also runs lm_update (single-rank fused mode)
   int use_loss;
   int use_edges;
+  int l2_hints;               // LM solves only: the bulk copies carry L2 eviction priorities (pv.resident_chunks)
   int loop_sweeps;            // > 1 (LOOP instantiations with a fused LM update only): the kernel runs up to that many LM
                               // iterations by itself -- sweep, reduce, lm_update, next sweep -- instead of one per launch
   unsigned long long* pose_ll;  // [16] looping multi-block grids: block 0 hands the next pose (7 doubles) and the `done` flag to
@@ -154,6 +156,23 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+// the same copy with an L2 eviction priority for the lines it reads (a policy made by createpolicy)
+__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                   smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+               : "memory");
+}
+__device__ __forceinline__ uint64_t policy_evict_last() {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ uint64_t policy_evict_first() {
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
 }
 
 __device__ __forceinline__ void st_relaxed_sys(unsigned long long* p, unsigned long long v) {
@@ -350,6 +369,11 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
   const int sweeps_max = (LOOP && args.loop_sweeps > 1 && MODE == kModeLM && args.lm != nullptr) ? args.loop_sweeps : 1;
   const int total_chunks = LOOP ? sweeps_max * n_chunks : n_chunks;
   int issued = 0, next_c = 0;  // next_c == issued mod n_chunks
+  // L2 residency during LM solves: every sweep reads the same bytes in the same order.  The last resident_chunks stages of the
+  // range are read with evict_last and stay in L2 from one sweep to the next; all other stages are read with evict_first, so
+  // that the stream does not push the resident share out.  The last stages, because the warps that finish late (the
+  // straggler tail, one or two stages in flight) then read from L2.  Only the eviction priority changes, not the arithmetic.
+  const bool l2_hints = args.l2_hints != 0 && pv.resident_chunks > 0;
   auto issue_one = [&](bool slot_was_read) {
     if (lane == 0) {
       const int c = LOOP ? next_c : issued, st = issued % NST;
@@ -358,9 +382,16 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       const int64_t src = p0 + (int64_t)c * CH;  // multiple of the stage size -> 1 KiB aligned
       if (slot_was_read) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       mbar_expect_tx(bars + st, (PLANAR ? 2 : 3) * CH * 8);
-      bulk_g2s(dst, pv.x + src, CH * 8, bars + st);
-      bulk_g2s(dst + CH, pv.y + src, CH * 8, bars + st);
-      if (!PLANAR) bulk_g2s(dst + 2 * CH, pv.z + src, CH * 8, bars + st);
+      if (l2_hints) {
+        const uint64_t pol = c >= n_chunks - pv.resident_chunks ? policy_evict_last() : policy_evict_first();
+        bulk_g2s_hint(dst, pv.x + src, CH * 8, bars + st, pol);
+        bulk_g2s_hint(dst + CH, pv.y + src, CH * 8, bars + st, pol);
+        if (!PLANAR) bulk_g2s_hint(dst + 2 * CH, pv.z + src, CH * 8, bars + st, pol);
+      } else {
+        bulk_g2s(dst, pv.x + src, CH * 8, bars + st);
+        bulk_g2s(dst + CH, pv.y + src, CH * 8, bars + st);
+        if (!PLANAR) bulk_g2s(dst + 2 * CH, pv.z + src, CH * 8, bars + st);
+      }
     }
     ++issued;
     if (LOOP && ++next_c == n_chunks) next_c = 0;
@@ -981,6 +1012,29 @@ __global__ void clc_flush_read_kernel(const double* buf, int64_t n, double* sink
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     acc += __ldcg(buf + i);
   if (acc == 123.456) *sink = acc;  // never true: keeps the loads alive
+}
+
+// End of an LM solve: the lines its sweeps read with evict_last go back to the normal priority, so that they do not outlive
+// the solve (other work on the GPU, the cold-L2 measurement hook).  One thread per 128-byte line of x in the resident share
+// of every warp's range (the stages clc_sweep_kernel marks, same range arithmetic); it demotes the same line of y and z.
+__global__ void clc_l2_demote_kernel(ProblemView pv, int64_t n_warps, int chunk) {
+  const int k = pv.resident_chunks;
+  const int64_t lines_per_warp = (int64_t)k * chunk / 16;  // 16 doubles per line
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_warps * lines_per_warp) return;
+  const int64_t w = t / lines_per_warp;
+  const int64_t P = pv.n_points;
+  int64_t p0 = w * pv.per_warp;
+  if (p0 > P) p0 = P;
+  int64_t p1 = p0 + pv.per_warp;
+  if (p1 > P) p1 = P;
+  const int64_t n_chunks = (p1 - p0 + chunk - 1) / chunk;
+  const int64_t c0 = n_chunks > k ? n_chunks - k : 0;  // first resident stage (a short last range may hold fewer than k)
+  const int64_t i = p0 + c0 * chunk + (t - w * lines_per_warp) * 16;
+  if (i >= p0 + n_chunks * chunk) return;
+  asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(pv.x + i) : "memory");
+  asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(pv.y + i) : "memory");
+  if (pv.z != nullptr) asm volatile("applypriority.global.L2::evict_normal [%0], 128;" ::"l"(pv.z + i) : "memory");
 }
 
 }  // namespace clc
