@@ -186,6 +186,8 @@ SIGNATURES = {
     "clc_problem_set_planar_mode": (C.c_int, [_P, C.c_int]),
     "clc_debug_pack": (C.c_int, [C.c_int64, C.POINTER(c_double_p), c_int64_p, C.c_int64, C.c_int64, C.c_int, c_double_p,
                                  C.POINTER(C.c_int)]),
+    "clc_debug_partition": (C.c_int, [_P, C.POINTER(C.c_int), c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                      C.POINTER(C.c_int)]),
     "clc_bench_h2d": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_solve_readback_bytes": (C.c_int64, []),
     "clc_host_alloc": (C.c_int, [C.POINTER(_P), C.c_int64]),

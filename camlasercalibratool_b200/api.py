@@ -223,6 +223,22 @@ class Problem:
         """1 = automatic (default): planar data runs the two-stream kernels; 0 = always the general kernels."""
         _lib.check(self._L.clc_problem_set_planar_mode(self._h, int(mode)), "clc_problem_set_planar_mode")
 
+    def partition(self, warp_table=True):
+        """The sweep kernel's static work partition for the active kernel family (test hook): dict with grid (blocks),
+        per_warp (points per warp range), stage (points per pipeline stage), resident_chunks (stages per warp kept in L2
+        during LM solves) and, with warp_table, warp_first_frame [grid * 12] (the frame holding each range's first point)."""
+        grid, per_warp, stage, resident = C.c_int(), C.c_int64(), C.c_int(), C.c_int()
+        L = self._L
+        _lib.check(L.clc_debug_partition(self._h, C.byref(grid), C.byref(per_warp), C.byref(stage), C.byref(resident), None),
+                   "clc_debug_partition")
+        out = dict(grid=grid.value, per_warp=per_warp.value, stage=stage.value, resident_chunks=resident.value)
+        if warp_table:
+            wff = np.empty(grid.value * 12, dtype=np.int32)
+            _lib.check(L.clc_debug_partition(self._h, None, None, None, None, wff.ctypes.data_as(C.POINTER(C.c_int))),
+                       "clc_debug_partition")
+            out["warp_first_frame"] = wff
+        return out
+
     def download(self):
         nf, npts, he = self.sizes()
         fp, off, pts = np.empty((nf, 7)), np.empty(nf + 1, dtype=np.int64), np.empty((npts, 3))

@@ -2055,6 +2055,24 @@ int clc_debug_pack(int64_t n_frames, const double* const* frame_points, const in
   return CLC_OK;
 }
 
+// test hook, read-only: the static work partition of the sweep kernels as partition() left it for the active kernel family,
+// and (warp_first_frame != nullptr, [grid * kWarps]) the warp start table clc_warp_table_kernel built from it
+int clc_debug_partition(const clc_problem* p, int* grid, int64_t* per_warp, int* stage_points, int* resident_chunks,
+                        int* warp_first_frame) {
+  if (!p) return fail(CLC_ERR_INVALID, "NULL problem");
+  if (grid) *grid = p->grid;
+  if (per_warp) *per_warp = p->per_warp;
+  if (stage_points) *stage_points = p->planar ? clc::kPlanarChunk : clc::kChunk;
+  if (resident_chunks) *resident_chunks = p->resident_chunks;
+  if (warp_first_frame) {
+    int rc = set_device(p);
+    if (rc != CLC_OK) return rc;
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
+    CLC_CUDA(cudaMemcpy(warp_first_frame, p->warp_first_frame, sizeof(int) * (size_t)p->grid * clc::kWarps, cudaMemcpyDeviceToHost));
+  }
+  return CLC_OK;
+}
+
 // statistics of the most recent host -> HBM upload of this process (measurement hook)
 int clc_upload_last_stats(double* total_ms, double* pack_wait_ms, int64_t* bytes_h2d, int* chunks, int* pack_threads,
                           int* direct) {

@@ -307,6 +307,11 @@ int clc_upload_last_stats(double* total_ms, double* pack_wait_ms, int64_t* bytes
  * pairs (xy != 0; *nonplanar = a z != 0 or NaN was met) or packed x,y,z. */
 int clc_debug_pack(int64_t n_frames, const double* const* frame_points, const int64_t* frame_counts, int64_t a, int64_t b,
                    int xy, double* out, int* nonplanar);
+/* Test hook, read-only: the static work partition of the sweep kernel for the problem's active kernel family -- launch grid
+ * (blocks), points per warp range, points per pipeline stage, stages per warp kept in L2 during LM solves -- and, when
+ * warp_first_frame is not NULL ([grid * 12] ints), the frame that holds the first point of every warp range. */
+int clc_debug_partition(const clc_problem* p, int* grid, int64_t* per_warp, int* stage_points, int* resident_chunks,
+                        int* warp_first_frame);
 /* Raw PCIe yardstick: `reps` host(pinned) -> device copies of `bytes` on `device`, each timed with CUDA events. */
 int clc_bench_h2d(int64_t bytes, int device, int reps, float* ms_each);
 /* Bytes clc_solve_lm reads back per solve (LM state + iteration trace). */
