@@ -136,6 +136,9 @@ TERMINATION = {
     6: "FAILURE",
 }
 
+# CLC_PATH_* (clc_debug_dispatch)
+PATHS = {1: "one_cluster", 2: "single_block", 3: "single_block_loop", 4: "multi_block", 5: "multi_block_loop"}
+
 # every symbol include/clc_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SIGNATURES = {
@@ -188,6 +191,8 @@ SIGNATURES = {
                                  C.POINTER(C.c_int)]),
     "clc_debug_partition": (C.c_int, [_P, C.POINTER(C.c_int), c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                       C.POINTER(C.c_int)]),
+    "clc_debug_dispatch": (C.c_int, [_P, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                     C.POINTER(C.c_int)]),
     "clc_bench_h2d": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_solve_readback_bytes": (C.c_int64, []),
     "clc_host_alloc": (C.c_int, [C.POINTER(_P), C.c_int64]),

@@ -239,6 +239,17 @@ class Problem:
             out["warp_first_frame"] = wff
         return out
 
+    def dispatch(self):
+        """The kernel each entry point runs on for this problem (test hook): dict with eval, information, closed_form and
+        solve, each one of "one_cluster", "single_block", "single_block_loop", "multi_block" or "multi_block_loop", and
+        small_shape = (threads per CTA, CTAs per cluster, residuals per thread) of the one-cluster kernel."""
+        paths = [C.c_int() for _ in range(4)]
+        shape = (C.c_int * 3)()
+        _lib.check(self._L.clc_debug_dispatch(self._h, *[C.byref(v) for v in paths], shape), "clc_debug_dispatch")
+        out = {k: _lib.PATHS[v.value] for k, v in zip(("eval", "information", "closed_form", "solve"), paths)}
+        out["small_shape"] = tuple(shape)
+        return out
+
     def download(self):
         nf, npts, he = self.sizes()
         fp, off, pts = np.empty((nf, 7)), np.empty(nf + 1, dtype=np.int64), np.empty((npts, 3))

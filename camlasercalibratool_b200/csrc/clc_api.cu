@@ -990,6 +990,21 @@ int clc_problem_download(const clc_problem* p, double* frame_pose, int64_t* offs
 // shards of an in-process multi-GPU group: enqueue on every device first (the fused exchange makes block 0 of every
 // device's kernel wait for its peers' kernels), then wait for all of them.
 
+// An LM-mode call runs on the one-cluster kernel K2 (clc_small.cuh) when its residuals (points, plus the edge residuals
+// when they are counted) fit the cluster and the problem has one rank; K1 serves everything else.
+static bool small_kernel_serves(const clc_problem* p, bool with_edges) {
+  return p->small_kernel && p->nranks <= 1 && p->n_points + (with_edges ? p->n_edges : 0) <= clc::kSmallMaxResiduals;
+}
+
+// A K1 solve runs the whole LM loop in one launch: always with CLC_LOOP_IN_KERNEL=2, by default on a single-block grid.
+static bool sweep_loops_in_kernel(const clc_problem* p) {
+  return p->loop_in_kernel >= 2 || (p->loop_in_kernel == 1 && p->grid == 1 && p->nranks <= 1);
+}
+
+// A solve runs lm_update at the tail of the sweep kernel (or inside K2) unless NCCL all-reduces the sums between kernels, in
+// which case K3 runs it as its own launch.
+static bool fused_lm_update(const clc_problem* p) { return p->nranks <= 1 || p->allreduce_mode == 1; }
+
 static int eval_enqueue(clc_problem* p, const double pose7[7], bool loss, bool edges, int mode, int count) {
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
@@ -1003,8 +1018,7 @@ static int eval_enqueue(clc_problem* p, const double pose7[7], bool loss, bool e
   }
   CLC_CUDA(cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
   const bool with_edges = edges && p->n_edges > 0;
-  if (mode == clc::kModeLM && p->small_kernel && p->nranks <= 1 &&
-      p->n_points + (with_edges ? p->n_edges : 0) <= clc::kSmallMaxResiduals) {
+  if (mode == clc::kModeLM && small_kernel_serves(p, with_edges)) {
     // a small problem: one evaluation by the one-cluster kernel (clc_small.cuh)
     const clc::ProblemView v = make_view(p);
     if (loss)
@@ -1216,7 +1230,7 @@ int solve_begin(clc_problem* p, const double pose7[7], const clc_lm_options& opt
   if (p->p2p_error) CLC_CUDA(cudaMemsetAsync(p->p2p_error, 0, sizeof(int), p->stream));  // a fresh solve starts clean
   CLC_CUDA(cudaMemcpyAsync(&p->lm->core, &p->h_lm->core, sizeof(clc::LmCore), cudaMemcpyHostToDevice, p->stream));
   CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
-  ctx->fused_update = (p->nranks <= 1) || p->allreduce_mode == 1;
+  ctx->fused_update = fused_lm_update(p);
   ctx->loss = p->use_loss != 0;
   ctx->edges = p->n_edges > 0;
   // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps
@@ -1326,8 +1340,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
   int launched = 0;
   // Small problems (the reference's own sizes): the whole solve in one launch of one thread-block cluster that keeps every
   // residual in registers (clc_small.cuh) -- no TMA rings, no gather, no global round trip between two LM iterations.
-  if (n == 1 && ps[0]->small_kernel && ps[0]->loop_in_kernel >= 1 && ps[0]->nranks <= 1 && ctx[0].fused_update &&
-      ps[0]->n_points + (ctx[0].edges ? ps[0]->n_edges : 0) <= clc::kSmallMaxResiduals) {
+  if (n == 1 && ps[0]->loop_in_kernel >= 1 && ctx[0].fused_update && small_kernel_serves(ps[0], ctx[0].edges)) {
     clc_problem* p = ps[0];
     rc = set_device(p);
     if (rc != CLC_OK) return rc;
@@ -1341,8 +1354,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
   }
   bool loop_launch = launched == 0;
   for (int g = 0; g < n; ++g)
-    loop_launch = loop_launch && ctx[g].fused_update &&
-                  (ps[g]->loop_in_kernel >= 2 || (ps[g]->loop_in_kernel == 1 && ps[g]->grid == 1 && ps[g]->nranks <= 1));
+    loop_launch = loop_launch && ctx[g].fused_update && sweep_loops_in_kernel(ps[g]);
   if (loop_launch) {
     // ONE launch per device runs the whole LM loop (sweep, reduce, [peer exchange,] lm_update, next sweep)
     for (int g = 0; g < n; ++g) {
@@ -2069,6 +2081,29 @@ int clc_debug_partition(const clc_problem* p, int* grid, int64_t* per_warp, int*
     if (rc != CLC_OK) return rc;
     CLC_CUDA(cudaStreamSynchronize(p->stream));
     CLC_CUDA(cudaMemcpy(warp_first_frame, p->warp_first_frame, sizeof(int) * (size_t)p->grid * clc::kWarps, cudaMemcpyDeviceToHost));
+  }
+  return CLC_OK;
+}
+
+// test hook, read-only: the kernel eval_enqueue and solve_all pick for this problem (the same predicates they use)
+int clc_debug_dispatch(const clc_problem* p, int* eval_path, int* information_path, int* closed_form_path, int* solve_path,
+                       int* small_shape) {
+  if (!p) return fail(CLC_ERR_INVALID, "NULL problem");
+  const int sweep = p->grid == 1 ? CLC_PATH_SINGLE_BLOCK : CLC_PATH_MULTI_BLOCK;
+  const bool edges = p->n_edges > 0;
+  const bool fused_update = fused_lm_update(p);
+  if (eval_path) *eval_path = small_kernel_serves(p, edges) ? CLC_PATH_ONE_CLUSTER : sweep;
+  if (information_path) *information_path = small_kernel_serves(p, false) ? CLC_PATH_ONE_CLUSTER : sweep;  // no edges
+  if (closed_form_path) *closed_form_path = sweep;
+  if (solve_path) {
+    if (p->loop_in_kernel >= 1 && fused_update && small_kernel_serves(p, edges)) *solve_path = CLC_PATH_ONE_CLUSTER;
+    else if (fused_update && sweep_loops_in_kernel(p)) *solve_path = sweep + 1;  // the looping variant of the same grid
+    else *solve_path = sweep;
+  }
+  if (small_shape) {
+    small_shape[0] = clc::kSmallThreads;
+    small_shape[1] = clc::kSmallCluster;
+    small_shape[2] = clc::kSmallItems;
   }
   return CLC_OK;
 }

@@ -312,6 +312,17 @@ int clc_debug_pack(int64_t n_frames, const double* const* frame_points, const in
  * warp_first_frame is not NULL ([grid * 12] ints), the frame that holds the first point of every warp range. */
 int clc_debug_partition(const clc_problem* p, int* grid, int64_t* per_warp, int* stage_points, int* resident_chunks,
                         int* warp_first_frame);
+/* The kernels clc_debug_dispatch reports. */
+#define CLC_PATH_ONE_CLUSTER 1        /* the one-cluster kernel: one launch per evaluation, or the whole LM solve */
+#define CLC_PATH_SINGLE_BLOCK 2       /* the sweep kernel on one block, one launch per evaluation / LM iteration */
+#define CLC_PATH_SINGLE_BLOCK_LOOP 3  /* the sweep kernel on one block, the whole LM loop in one launch */
+#define CLC_PATH_MULTI_BLOCK 4        /* the sweep kernel on several blocks, one launch per evaluation / LM iteration */
+#define CLC_PATH_MULTI_BLOCK_LOOP 5   /* the persistent looping grid of the sweep kernel, the whole LM loop in one launch */
+/* Test hook, read-only: the kernel (CLC_PATH_*) that clc_eval, clc_information, clc_closed_form and clc_solve_lm run on for
+ * this problem under the knobs read at its creation, and (small_shape != NULL, [3] ints) the one-cluster kernel's shape:
+ * threads per CTA, CTAs per cluster, residuals per thread.  Any pointer may be NULL. */
+int clc_debug_dispatch(const clc_problem* p, int* eval_path, int* information_path, int* closed_form_path, int* solve_path,
+                       int* small_shape);
 /* Raw PCIe yardstick: `reps` host(pinned) -> device copies of `bytes` on `device`, each timed with CUDA events. */
 int clc_bench_h2d(int64_t bytes, int device, int reps, float* ms_each);
 /* Bytes clc_solve_lm reads back per solve (LM state + iteration trace). */

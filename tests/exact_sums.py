@@ -129,12 +129,23 @@ def _residual_blocks(frame_pose, offsets, points, edge_points):
 
 def lm_sums(frame_pose, offsets, points, pose7, use_loss=True, cauchy_a=0.05, edge_points=None):
     """The 28 sums of one LM sweep (21 upper-triangle H, 6 g, cost) in long double, and their magnitudes A_k (float64)."""
+    return lm_sums_of_blocks(_residual_blocks(frame_pose, offsets, points, edge_points), pose7, use_loss, cauchy_a)
+
+
+def lm_sums_of_residuals(plane, point, s2, pose7, use_loss=True, cauchy_a=0.05):
+    """lm_sums over an explicit residual list: plane [k,4], point [k,3], s2 [k] (the residual's 1 / #points)."""
+    blocks = ((plane[a:a + CHUNK].astype(LD), np.asarray(point[a:a + CHUNK]).astype(LD), s2[a:a + CHUNK].astype(LD))
+              for a in range(0, len(s2), CHUNK))
+    return lm_sums_of_blocks(blocks, pose7, use_loss, cauchy_a)
+
+
+def lm_sums_of_blocks(blocks, pose7, use_loss=True, cauchy_a=0.05):
     pose = np.asarray(pose7, dtype=np.float64).astype(LD)
     R, t = _rot(pose[3:7]), pose[:3]
     a2 = LD(cauchy_a) * LD(cauchy_a)
     val = np.zeros(28, dtype=LD)
     mag = np.zeros(28)
-    for plane, p, s2 in _residual_blocks(frame_pose, offsets, points, edge_points):
+    for plane, p, s2 in blocks:
         n, d = plane[:, :3], plane[:, 3]
         m = n @ R                                   # R^T n
         c = n @ t + d
