@@ -11,6 +11,7 @@ from .api import (  # noqa: F401
     LineFittingCeres,
     ClcError,
     Comm,
+    FRAME_ROW_DTYPE,
     Group,
     Oberserve,
     Problem,
@@ -18,6 +19,7 @@ from .api import (  # noqa: F401
     comm_unique_id,
     debug_pack,
     default_options,
+    frame_influence,
     launch_count,
     marshal,
     pose7_to_T,
@@ -28,4 +30,5 @@ from .api import (  # noqa: F401
 __all__ = [
     "CamLaserCalClosedSolution", "CamLaserCalibration", "LineFittingCeres", "ClcError", "Comm", "Group", "Oberserve", "Problem", "T_to_pose7",
     "comm_unique_id", "default_options", "launch_count", "marshal", "pose7_to_T", "shard_range", "debug_pack", "upload_stats",
+    "FRAME_ROW_DTYPE", "frame_influence",
 ]

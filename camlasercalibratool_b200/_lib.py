@@ -126,6 +126,22 @@ class LmSummary(C.Structure):
     ]
 
 
+class FrameRow(C.Structure):
+    """clc_frame_row: one frame of clc_frame_report."""
+    _fields_ = [
+        ("n_points", C.c_int64),
+        ("cost", C.c_double),
+        ("chi", C.c_double),
+        ("mean_e", C.c_double),
+        ("rms_e", C.c_double),
+        ("max_abs_e", C.c_double),
+        ("mean_weight", C.c_double),
+        ("edge_e", C.c_double * 2),
+        ("H21", C.c_double * 21),
+        ("g6", C.c_double * 6),
+    ]
+
+
 TERMINATION = {
     0: "RUNNING",
     1: "CONVERGENCE_FUNCTION",
@@ -157,6 +173,7 @@ SIGNATURES = {
     "clc_group_solve_lm": (C.c_int, [_P, c_double_p, C.POINTER(LmOptions), C.POINTER(LmSummary), C.POINTER(LmIteration), C.c_int]),
     "clc_group_information": (C.c_int, [_P, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     "clc_group_closed_form": (C.c_int, [_P, c_double_p, C.POINTER(C.c_int), c_double_p, c_double_p]),
+    "clc_group_frame_report": (C.c_int, [_P, c_double_p, _P]),
     "clc_default_devices": (C.c_int, [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     "clc_upload_last_stats": (C.c_int, [c_double_p, c_double_p, c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "clc_problem_destroy": (C.c_int, [_P]),
@@ -167,6 +184,7 @@ SIGNATURES = {
     "clc_solve_lm": (C.c_int, [_P, c_double_p, C.POINTER(LmOptions), C.POINTER(LmSummary), C.POINTER(LmIteration), C.c_int]),
     "clc_information": (C.c_int, [_P, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     "clc_closed_form": (C.c_int, [_P, c_double_p, C.POINTER(C.c_int), c_double_p, c_double_p]),
+    "clc_frame_report": (C.c_int, [_P, c_double_p, _P]),
     "clc_problem_line_fit": (C.c_int, [_P, c_double_p, C.c_int, c_double_p]),
     "clc_line_fit_points": (C.c_int, [c_double_p, C.c_int64, c_double_p, C.c_int]),
     "clc_scan_segments": (C.c_int, [C.POINTER(C.c_float), C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_double,
@@ -184,6 +202,7 @@ SIGNATURES = {
     "clc_problem_attach_comm": (C.c_int, [_P, _P]),
     "clc_problem_set_allreduce_mode": (C.c_int, [_P, C.c_int]),
     "clc_bench_eval": (C.c_int, [_P, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
+    "clc_bench_frame_report": (C.c_int, [_P, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_problem_algorithmic_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_streamed_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_set_planar_mode": (C.c_int, [_P, C.c_int]),

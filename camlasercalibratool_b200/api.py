@@ -116,6 +116,50 @@ def _synthetic_desc(n_frames_total, beams, seed, sigma, with_edges, frame_begin,
     return d
 
 
+# clc_frame_row (include/clc_b200.h) as a numpy record: Problem.frame_report / Group.frame_report return arrays of it
+FRAME_ROW_DTYPE = np.dtype([("n_points", np.int64), ("cost", np.float64), ("chi", np.float64), ("mean_e", np.float64),
+                            ("rms_e", np.float64), ("max_abs_e", np.float64), ("mean_weight", np.float64),
+                            ("edge_e", np.float64, (2,)), ("H21", np.float64, (21,)), ("g6", np.float64, (6,))])
+assert FRAME_ROW_DTYPE.itemsize == C.sizeof(_lib.FrameRow)
+
+
+def _frame_report(fn, handle, n_frames, pose7, what):
+    pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+    rows = np.zeros(n_frames, dtype=FRAME_ROW_DTYPE)
+    _lib.check(fn(handle, _dp(pose7), rows.ctypes.data_as(C.c_void_p)), what)
+    return rows
+
+
+def frame_influence(report, H, g):
+    """One-step leave-one-frame-out estimate of how far the extrinsic moves without each frame.
+
+    report: a frame report (Problem.frame_report) and H [6,6], g [6]: clc_eval's at the same pose.  For every frame f,
+    delta_f = -(H - H_f)^-1 (g - g_f) is ONE Gauss-Newton step of the problem without frame f from this pose -- an estimate, not
+    a re-solve: it is close to the re-solved extrinsic's move when the pose is near the optimum and frame f does not change
+    which residuals the Cauchy loss down-weights.  delta_f is a pose increment in the solver's parameterisation (translation,
+    then rotation vector; pose_plus).  Frames whose H - H_f is numerically singular (the frame alone pins a direction) get NaN.
+    Batched 6x6 solves on the host, O(n_frames).
+
+    Returns (delta [N, 6], translation norm [N] in metres, rotation norm [N] in radians)."""
+    iu = np.triu_indices(6)
+    N = len(report)
+    Hf = np.zeros((N, 6, 6))
+    Hf[:, iu[0], iu[1]] = report["H21"]
+    Hf = Hf + np.triu(Hf, 1).transpose(0, 2, 1)
+    A = np.asarray(H, dtype=np.float64)[None] - Hf
+    b = np.asarray(g, dtype=np.float64)[None] - report["g6"]
+    delta = np.full((N, 6), np.nan)
+    with np.errstate(invalid="ignore"):
+        finite = np.all(np.isfinite(A.reshape(N, -1)), axis=1) & np.all(np.isfinite(b), axis=1)
+    if np.any(finite):
+        sv = np.linalg.svd(A[finite], compute_uv=False)
+        regular = sv[:, -1] > sv[:, 0] * 6 * np.finfo(np.float64).eps  # numpy's matrix_rank threshold
+        idx = np.nonzero(finite)[0][regular]
+        if idx.size:
+            delta[idx] = -np.linalg.solve(A[idx], b[idx][..., None])[..., 0]
+    return delta, np.linalg.norm(delta[:, :3], axis=1), np.linalg.norm(delta[:, 3:], axis=1)
+
+
 def default_options(**kw) -> LmOptions:
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
@@ -288,6 +332,12 @@ class Problem:
                    "clc_information")
         return H, b, chi.value, sv
 
+    def frame_report(self, pose7):
+        """Every frame's residual statistics and share of the normal equations at pose7 (clc_frame_report): a numpy record
+        array of FRAME_ROW_DTYPE, one row per frame.  Rows sum to eval()'s cost, H (upper triangle) and g, and their chi to
+        information()'s chi."""
+        return _frame_report(self._L.clc_frame_report, self._h, self.sizes()[0], pose7, "clc_frame_report")
+
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()
         _lib.check(self._L.clc_closed_form(self._h, _dp(T), C.byref(un), _dp(AtA), _dp(Atb)), "clc_closed_form")
@@ -316,6 +366,13 @@ class Problem:
         pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_eval(self._h, _dp(pose7), int(n), int(bool(flush_l2)), ms), "clc_bench_eval")
+        return np.array(ms[:], dtype=np.float64)
+
+    def bench_frame_report(self, pose7, n, flush_l2=True):
+        """Device time of n frame reports (per-frame sweep + split-frame fix-up, without the copy of the rows), ms each."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_frame_report(self._h, _dp(pose7), int(n), int(bool(flush_l2)), ms), "clc_bench_frame_report")
         return np.array(ms[:], dtype=np.float64)
 
 
@@ -410,6 +467,10 @@ class Group:
         _lib.check(self._L.clc_group_information(self._h, _dp(pose7), _dp(H), _dp(b), C.byref(chi), _dp(sv), _dp(self.last_V)),
                    "clc_group_information")
         return H, b, chi.value, sv
+
+    def frame_report(self, pose7):
+        """Problem.frame_report over every shard, rows in the global frame order (clc_group_frame_report)."""
+        return _frame_report(self._L.clc_group_frame_report, self._h, self.sizes()[1], pose7, "clc_group_frame_report")
 
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()

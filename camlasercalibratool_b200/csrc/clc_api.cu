@@ -10,9 +10,11 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -317,8 +319,10 @@ int set_device(const clc_problem* p) {
 
 // one K1 launch on the problem's stream
 // collective: the sums of this launch are to be all-reduced (in-kernel when the peer path is active)
+// kModeFrames: frame_rows / frame_slots receive the per-frame report (clc_frame_fixup_kernel finishes it)
 int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* d_pose, const int* d_done,
-                 clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false) {
+                 clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false,
+                 double* frame_rows = nullptr, double* frame_slots = nullptr) {
   clc::SweepArgs a;
   a.pose7 = d_pose;
   a.done = d_done;
@@ -336,6 +340,8 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   a.rank = 0;
   a.seq_counter = nullptr;
   a.error = p->p2p_error;
+  a.frame_rows = frame_rows;
+  a.frame_slots = frame_slots;
   if (p->nranks > 1 && p->allreduce_mode == 1 && collective) {
     clc_comm* c = p->comm_obj;
     a.nranks = c->nranks;
@@ -348,7 +354,7 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)p->grid);
   cfg.blockDim = dim3(clc::kThreads);
-  cfg.dynamicSmemBytes = clc::dyn_smem_bytes(p->planar);
+  cfg.dynamicSmemBytes = mode == clc::kModeFrames ? clc::frames_smem_bytes(p->planar) : clc::dyn_smem_bytes(p->planar);
   cfg.stream = p->stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -357,7 +363,16 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   cfg.numAttrs = 1;
   cudaError_t le;
   if (!p->planar && p->z == nullptr) return fail(CLC_ERR_INVALID, "internal: general sweep without a z stream");
-  if (mode == clc::kModeClosedForm) {
+  if (mode == clc::kModeFrames) {
+    // the per-frame report: no LM state, no L2 hints, never collective
+    if (frame_rows == nullptr || frame_slots == nullptr || d_lm != nullptr || loop_sweeps > 1 || a.nranks > 1)
+      return fail(CLC_ERR_INVALID, "internal: bad per-frame sweep");
+    void (*fn)(clc::ProblemView, clc::SweepArgs) =
+        loss ? (p->planar ? clc::clc_sweep_kernel<true, clc::kModeFrames, true> : clc::clc_sweep_kernel<true, clc::kModeFrames, false>)
+             : (p->planar ? clc::clc_sweep_kernel<false, clc::kModeFrames, true> : clc::clc_sweep_kernel<false, clc::kModeFrames, false>);
+    CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+    le = cudaLaunchKernelEx(&cfg, fn, v, a);
+  } else if (mode == clc::kModeClosedForm) {
     le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeClosedForm, true>, v, a)
                    : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeClosedForm, false>, v, a);
   } else if (loop_sweeps > 1) {
@@ -1171,6 +1186,99 @@ int clc_closed_form(clc_problem* p, double Tlc[16], int* unobservable, double At
   if (rc != CLC_OK) return rc;
   closed_form_post(p->h_sums, Tlc, unobservable, AtA81, Atb9);
   return CLC_OK;
+}
+
+// ---- the per-frame report ------------------------------------------------------------------------------------------
+// Every problem size runs it on the sweep kernel K1 (a kModeFrames sweep, then clc_frame_fixup_kernel for the frames that cross a
+// warp-range end), with the kernel family eval uses.  The rows stay on the device until one copy into the caller's array.
+
+static_assert(sizeof(clc_frame_row) == sizeof(double) * clc::kRowDoubles, "clc_frame_row is the kernels' row");
+static_assert(offsetof(clc_frame_row, n_points) == 8 * clc::kRowN && offsetof(clc_frame_row, cost) == 8 * clc::kRowCost &&
+                  offsetof(clc_frame_row, chi) == 8 * clc::kRowChi && offsetof(clc_frame_row, mean_e) == 8 * clc::kRowMeanE &&
+                  offsetof(clc_frame_row, rms_e) == 8 * clc::kRowRmsE && offsetof(clc_frame_row, max_abs_e) == 8 * clc::kRowMaxE &&
+                  offsetof(clc_frame_row, mean_weight) == 8 * clc::kRowMeanW &&
+                  offsetof(clc_frame_row, edge_e) == 8 * clc::kRowEdgeE && offsetof(clc_frame_row, H21) == 8 * clc::kRowH &&
+                  offsetof(clc_frame_row, g6) == 8 * clc::kRowG,
+              "clc_frame_row field offsets");
+
+namespace {
+
+struct FrameReportBuffers {
+  double* rows = nullptr;   // [n_frames * kRowDoubles]
+  double* slots = nullptr;  // [grid * kWarps * 2 * kSlotDoubles]
+};
+
+int frame_report_alloc(clc_problem* p, FrameReportBuffers* b) {
+  const size_t n_slots = (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles;
+  CLC_CUDA(cudaMallocAsync(&b->rows, sizeof(double) * clc::kRowDoubles * (size_t)std::max<int64_t>(p->n_frames, 1), p->stream));
+  CLC_CUDA(cudaMallocAsync(&b->slots, sizeof(double) * n_slots, p->stream));
+  return CLC_OK;
+}
+
+void frame_report_free(clc_problem* p, FrameReportBuffers* b) {
+  if (b->rows) cudaFreeAsync(b->rows, p->stream);
+  if (b->slots) cudaFreeAsync(b->slots, p->stream);
+  b->rows = b->slots = nullptr;
+}
+
+// the report at the pose in p->pose: the per-frame sweep, then the fix-up of split and empty frames
+int frame_report_launch(clc_problem* p, const FrameReportBuffers& b) {
+  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  int rc = launch_sweep(p, clc::kModeFrames, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false, /*pdl=*/false,
+                        /*loop_sweeps=*/1, /*l2_hints=*/false, b.rows, b.slots);
+  if (rc != CLC_OK) return rc;
+  const int threads = 256;
+  const unsigned blocks = (unsigned)((p->n_frames + threads - 1) / threads);
+  const clc::ProblemView v = make_view(p);
+  if (loss)
+    clc::clc_frame_fixup_kernel<true><<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
+  else
+    clc::clc_frame_fixup_kernel<false><<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the reports of the shards ps[0..n) into rows, shard after shard (the global frame order of a group)
+int frame_report_all(clc_problem* const* ps, int n, const double pose7[7], clc_frame_row* rows) {
+  std::vector<FrameReportBuffers> bufs((size_t)n);
+  int rc = CLC_OK;
+  for (int g = 0; g < n && rc == CLC_OK; ++g) {  // enqueue on every device first, then collect
+    clc_problem* p = ps[g];
+    if (p->n_frames == 0) continue;
+    rc = set_device(p);
+    if (rc != CLC_OK) break;
+    double* h_pose = p->pinned->pose;
+    for (int i = 0; i < 7; ++i) h_pose[i] = pose7[i];
+    if (cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream) != cudaSuccess) {
+      rc = fail(CLC_ERR_CUDA, "pose upload failed");
+      break;
+    }
+    rc = frame_report_alloc(p, &bufs[g]);
+    if (rc == CLC_OK) rc = frame_report_launch(p, bufs[g]);
+  }
+  int64_t first = 0;
+  for (int g = 0; g < n; ++g) {
+    clc_problem* p = ps[g];
+    if (bufs[g].rows != nullptr) {
+      cudaSetDevice(p->device);
+      if (rc == CLC_OK) {
+        cudaError_t e = cudaMemcpyAsync(rows + first, bufs[g].rows, sizeof(clc_frame_row) * (size_t)p->n_frames,
+                                        cudaMemcpyDeviceToHost, p->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
+        if (e != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("frame report: ") + cudaGetErrorString(e));
+      }
+      frame_report_free(p, &bufs[g]);
+    }
+    first += p->n_frames;
+  }
+  return rc;
+}
+
+}  // namespace
+
+int clc_frame_report(clc_problem* p, const double pose7[7], clc_frame_row* rows) {
+  if (!p || !pose7 || (!rows && p->n_frames > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
+  return frame_report_all(&p, 1, pose7, rows);
 }
 
 // ---- the on-device LM solve ------------------------------------------------------------------------------------
@@ -2007,6 +2115,11 @@ int clc_group_closed_form(clc_group* g, double Tlc16[16], int* unobservable, dou
   return CLC_OK;
 }
 
+int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* rows) {
+  if (!g || g->problems.empty() || !pose7 || (!rows && g->n_frames > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
+  return frame_report_all(g->problems.data(), (int)g->problems.size(), pose7, rows);
+}
+
 int clc_group_solve_lm(clc_group* g, double pose7[7], const clc_lm_options* opt, clc_lm_summary* summary,
                        clc_lm_iteration* trace, int trace_cap) {
   if (!g || g->problems.empty() || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
@@ -2122,45 +2235,83 @@ int clc_upload_last_stats(double* total_ms, double* pack_wait_ms, int64_t* bytes
 
 // ---- measurement hooks -------------------------------------------------------------------------------------------
 
+namespace {
+
+// The L2 flush of the measurement hooks.  The flush kernels run with the timed kernel's shared-memory carve-out (CLC_FLUSH_SMEM=0
+// disables): an SM that has to switch its L1/shared split between two kernels drains first, and in the LM loop the sweeps follow
+// each other with the same split -- the timed launch should not pay a reconfiguration the product never sees.
+int bench_flush_prepare(clc_problem* p, int flush_l2, int smem, int* flush_smem) {
+  *flush_smem = smem;
+  if (!flush_l2) return CLC_OK;
+  if (!p->flush_buf) {
+    p->flush_n = ((int64_t)256 << 20) / sizeof(double);  // 256 MiB > 50 MB of L2
+    CLC_CUDA(cudaMallocAsync(&p->flush_buf, sizeof(double) * p->flush_n, p->stream));
+  }
+  if (const char* env = std::getenv("CLC_FLUSH_SMEM")) {
+    if (std::atoi(env) == 0) *flush_smem = 0;
+  }
+  if (*flush_smem > 0) {
+    CLC_CUDA(cudaFuncSetAttribute(clc::clc_flush_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, *flush_smem));
+    CLC_CUDA(cudaFuncSetAttribute(clc::clc_flush_read_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, *flush_smem));
+  }
+  return CLC_OK;
+}
+
+int bench_flush(clc_problem* p, int i, int flush_smem) {
+  clc::clc_flush_kernel<<<p->num_sms, 1024, flush_smem, p->stream>>>(p->flush_buf, p->flush_n, (double)i);
+  CLC_LAUNCH_CHECK();
+  clc::clc_flush_read_kernel<<<p->num_sms, 1024, flush_smem, p->stream>>>(p->flush_buf, p->flush_n, p->flush_buf);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// n launches of `launch` on the problem's stream, each bracketed by its own CUDA events (the L2 flush outside the brackets)
+int bench_loop(clc_problem* p, int n, int flush_l2, int flush_smem, float* ms_each, const std::function<int()>& launch) {
+  std::vector<cudaEvent_t> ev(2 * (size_t)n);
+  for (auto& e : ev) CLC_CUDA(cudaEventCreate(&e));
+  int rc = CLC_OK;
+  for (int i = 0; i < n && rc == CLC_OK; ++i) {
+    if (flush_l2) rc = bench_flush(p, i, flush_smem);
+    if (rc == CLC_OK) rc = cudaEventRecord(ev[2 * i], p->stream) == cudaSuccess ? launch() : fail(CLC_ERR_CUDA, "cudaEventRecord");
+    if (rc == CLC_OK && cudaEventRecord(ev[2 * i + 1], p->stream) != cudaSuccess) rc = fail(CLC_ERR_CUDA, "cudaEventRecord");
+  }
+  cudaError_t e = cudaStreamSynchronize(p->stream);
+  for (int i = 0; i < n && rc == CLC_OK && e == cudaSuccess; ++i) e = cudaEventElapsedTime(&ms_each[i], ev[2 * i], ev[2 * i + 1]);
+  for (auto& x : ev) cudaEventDestroy(x);
+  if (rc == CLC_OK && e != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("bench: ") + cudaGetErrorString(e));
+  return rc;
+}
+
+}  // namespace
+
 int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each) {
   if (!p || !pose7 || n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
-  if (flush_l2 && !p->flush_buf) {
-    p->flush_n = ((int64_t)256 << 20) / sizeof(double);  // 256 MiB > 50 MB of L2
-    CLC_CUDA(cudaMallocAsync(&p->flush_buf, sizeof(double) * p->flush_n, p->stream));
-  }
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
-  std::vector<cudaEvent_t> ev(2 * (size_t)n);
-  for (auto& e : ev) CLC_CUDA(cudaEventCreate(&e));
   const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
-  // The flush kernels run with the sweep kernel's shared-memory carve-out (CLC_FLUSH_SMEM=0 disables): an SM that has to
-  // switch its L1/shared split between two kernels drains first, and in the LM loop the sweeps follow each other with
-  // the same split -- the timed launch should not pay a reconfiguration the product never sees.
-  int flush_smem = clc::dyn_smem_bytes(p->planar);
-  if (const char* env = std::getenv("CLC_FLUSH_SMEM")) {
-    if (std::atoi(env) == 0) flush_smem = 0;
-  }
-  if (flush_l2 && flush_smem > 0) {
-    CLC_CUDA(cudaFuncSetAttribute(clc::clc_flush_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, flush_smem));
-    CLC_CUDA(cudaFuncSetAttribute(clc::clc_flush_read_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, flush_smem));
-  }
-  for (int i = 0; i < n; ++i) {
-    if (flush_l2) {
-      clc::clc_flush_kernel<<<p->num_sms, 1024, flush_smem, p->stream>>>(p->flush_buf, p->flush_n, (double)i);
-      CLC_LAUNCH_CHECK();
-      clc::clc_flush_read_kernel<<<p->num_sms, 1024, flush_smem, p->stream>>>(p->flush_buf, p->flush_n, p->flush_buf);
-      CLC_LAUNCH_CHECK();
-    }
-    CLC_CUDA(cudaEventRecord(ev[2 * i], p->stream));
-    rc = launch_sweep(p, clc::kModeLM, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false);
-    if (rc != CLC_OK) return rc;
-    CLC_CUDA(cudaEventRecord(ev[2 * i + 1], p->stream));
-  }
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
-  for (int i = 0; i < n; ++i) CLC_CUDA(cudaEventElapsedTime(&ms_each[i], ev[2 * i], ev[2 * i + 1]));
-  for (auto& e : ev) cudaEventDestroy(e);
-  return CLC_OK;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
+    return launch_sweep(p, clc::kModeLM, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false);
+  });
+}
+
+int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each) {
+  if (!p || !pose7 || n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  if (p->n_frames == 0) return fail(CLC_ERR_INVALID, "the problem has no frames");
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::frames_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
+  CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
+  FrameReportBuffers b;
+  rc = frame_report_alloc(p, &b);
+  if (rc == CLC_OK) rc = bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return frame_report_launch(p, b); });
+  frame_report_free(p, &b);
+  return rc;
 }
 
 // Profiling hook (not part of the reference-facing surface): one sweep with per-block globaltimer stamps.

@@ -124,6 +124,25 @@ CLC_HD void accumulate_residual(const PoseConsts& pc, const double* plane, doubl
   acc[27] += cost;
 }
 
+// One board-edge residual (plane = an edge plane, pt = its edge point) expanded through its moments into out[28], as the edge
+// tail of the sweep kernel does; returns the raw distance e.  s2 = 1/#points of the frame.
+CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const double* pt, double s2, bool use_loss, double a2,
+                            double inv_a2, double* out) {
+  double m[3], c;
+  frame_consts(pc, plane, m, &c);
+  const double x = pt[0], y = pt[1], z = pt[2];
+  const double e = fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
+  double w = 1.0, cost_term = e * e;
+  if (use_loss) {
+    const double u = fma(e * inv_a2, e, 1.0);
+    w = 1.0 / u;
+    cost_term = log(u);
+  }
+  const double S[10] = {w, w * x, w * y, w * z, w * x * x, w * x * y, w * x * z, w * y * y, w * y * z, w * z * z};
+  expand_lm(plane, m, c, s2, S, use_loss, cost_term, a2, out);
+  return e;
+}
+
 // Closed-form initialisation (reference src/LaseCamCalCeres.cpp:144-161): row A_k = n (x) (x, y, 1), b_k = -d, so
 // A^T A = sum_frames M (x) n n^T with M = sum_j pbar pbar^T (unweighted moments, z ignored) and
 // A^T b = sum_frames -d (M e_3) (x) n.   out[54] = 45 upper-tri of the 9x9 (row-major) then 9 of A^T b.

@@ -11,6 +11,7 @@
 
 #include "clc_camera.cuh"
 #include "clc_expand.cuh"
+#include "clc_frames.cuh"
 #include "clc_lm.cuh"
 
 namespace clc {
@@ -68,7 +69,15 @@ __host__ __device__ constexpr int dyn_smem_bytes(bool planar) {
   return kWarps * ring_doubles_per_warp(planar) * 8 + kWarps * kTileDoublesPerWarp * 8 + kWarps * kBarsPerWarp * 8;
 }
 
-enum SweepMode { kModeLM = 0, kModeClosedForm = 1 };
+// per-frame report mode: the tile keeps 3 more doubles per parked piece (sum e, sum e^2, max |e|) behind the mbarriers
+constexpr int kFrameTileDoublesPerWarp = 32 * 3;
+__host__ __device__ constexpr int frames_smem_bytes(bool planar) {
+  return dyn_smem_bytes(planar) + kWarps * kFrameTileDoublesPerWarp * 8;
+}
+
+// kModeFrames: the per-frame report (clc_frame_report) -- every frame's residual statistics and its share of the normal
+// equations go to a row of their own instead of being summed
+enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2 };
 
 // Device-resident problem (read-only for the sweeps).
 struct ProblemView {
@@ -116,6 +125,9 @@ struct SweepArgs {
   unsigned long long* peer_mailbox[kMaxRanks];  // peer_mailbox[r]: rank r's mailbox (IPC-mapped),
                                                 // [2 parity][nranks source][kMailboxSlot values][2 words]
   int* error;                             // set to 1 on a peer time-out
+  // kModeFrames only
+  double* frame_rows;   // [n_frames * kRowDoubles] the report rows of the frames that lie in one warp range
+  double* frame_slots;  // [total warps * 2 * kSlotDoubles] head / tail pieces of split frames (clc_frames.cuh)
 };
 
 // ---- small device helpers ---------------------------------------------------------------------------------
@@ -309,6 +321,65 @@ __device__ __forceinline__ void renormalise(Moments& a) {
   a.prod = __hiloint2double(hi - (ex << 20), __double2loint(a.prod));
 }
 
+// kModeFrames: the unweighted per-point statistics of a piece, next to its Moments (per lane)
+struct FrameSums {
+  double se, se2, emax;  // sum e, sum e^2, max |e| (NaN kept) of the raw distances
+};
+
+__device__ __forceinline__ void frame_sums_clear(FrameSums& s) { s.se = s.se2 = s.emax = 0.0; }
+
+// the same two points as process2 (the same e, rounded the same way)
+template <bool PLANAR>
+__device__ __forceinline__ void frame_sums2(FrameSums& s, const double2 X, const double2 Y, const double2 Z, bool v0, bool v1,
+                                            double m0, double m1, double m2, double c) {
+  const double e0 = fma(m0, X.x, fma(m1, Y.x, PLANAR ? c : fma(m2, Z.x, c)));
+  const double e1 = fma(m0, X.y, fma(m1, Y.y, PLANAR ? c : fma(m2, Z.y, c)));
+  const double d0 = v0 ? e0 : 0.0, d1 = v1 ? e1 : 0.0;
+  s.se += d0;
+  s.se += d1;
+  s.se2 = fma(d0, d0, s.se2);
+  s.se2 = fma(d1, d1, s.se2);
+  s.emax = nan_max(s.emax, fabs(d0));
+  s.emax = nan_max(s.emax, fabs(d1));
+}
+
+// Expands the summed pieces of frame f into its report row (clc_frames.cuh layout): S = the 10 weighted moments, cost_term as
+// expand_lm takes it, se / se2 / emax the unweighted statistics of its n points.  The frame's two edge residuals (edges) are
+// expanded exactly as K1's edge tail does and added to the row.
+__device__ __forceinline__ void frame_row_write(const ProblemView& pv, const PoseConsts& pc, int64_t f, int64_t n, const double* S,
+                                                double cost_term, double se, double se2, double emax, bool loss, bool edges,
+                                                double* row) {
+  double plane[4], m[3], c;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) plane[k] = pv.plane[f * 4 + k];
+  frame_consts(pc, plane, m, &c);
+  const double s2 = 1.0 / (double)(pv.offsets[f + 1] - pv.offsets[f]);
+  double out[kNumSums];
+#pragma unroll
+  for (int k = 0; k < kNumSums; ++k) out[k] = 0.0;
+  expand_lm(plane, m, c, s2, S, loss, cost_term, pv.a2, out);
+  double ee[2] = {0.0, 0.0};
+  if (edges) {
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+      ee[k] = edge_residual(pc, pv.edge_plane + (2 * f + k) * 4, pv.edge_pt + (2 * f + k) * 3, s2, loss, pv.a2, pv.inv_a2, out);
+  }
+  const double dn = (double)n;
+  row[kRowN] = __longlong_as_double(n);
+  row[kRowCost] = out[27];
+  row[kRowChi] = s2 * se2;
+  row[kRowMeanE] = se / dn;
+  row[kRowRmsE] = sqrt(se2 / dn);
+  row[kRowMaxE] = emax;
+  row[kRowMeanW] = S[0] / dn;
+  row[kRowEdgeE] = ee[0];
+  row[kRowEdgeE + 1] = ee[1];
+#pragma unroll
+  for (int k = 0; k < 21; ++k) row[kRowH + k] = out[k];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) row[kRowG + k] = out[21 + k];
+}
+
 // ---- K1: the fused sweep -------------------------------------------------------------------------------------
 //
 // Work decomposition: the P points are cut into equal contiguous ranges (a multiple of 128 points), one per warp of
@@ -327,7 +398,7 @@ __device__ __forceinline__ void renormalise(Moments& a) {
 template <bool LOSS, int MODE, bool PLANAR, bool LOOP = false>
 __global__ void __launch_bounds__(kThreads, kBlocksPerSM)
 clc_sweep_kernel(ProblemView pv, SweepArgs args) {
-  constexpr int NOUT = (MODE == kModeLM) ? kNumSums : kMaxOut;
+  constexpr int NOUT = (MODE == kModeClosedForm) ? kMaxOut : kNumSums;
   // planar: two coordinate streams per stage; stages of kPlanarChunk points keep the bytes in flight per warp the same
   constexpr int NST = PLANAR ? kPlanarStages : kStages;
   constexpr int CH = PLANAR ? kPlanarChunk : kChunk;  // points per stage
@@ -363,6 +434,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
   double* ring = reinterpret_cast<double*>(s_dyn) + warp * RING;
   double* tile = reinterpret_cast<double*>(s_dyn) + kWarps * RING + warp * kTileDoublesPerWarp;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_dyn + (size_t)kWarps * (RING + kTileDoublesPerWarp) * 8) + warp * kBarsPerWarp;
+  // kModeFrames: sum e, sum e^2, max |e| of every parked piece (tile row r -> ftile[3 r ..])
+  double* ftile = reinterpret_cast<double*>(s_dyn + dyn_smem_bytes(PLANAR)) + warp * kFrameTileDoublesPerWarp;
 
   // Stage slots and mbarrier phases follow a running count of issued stages (`issued`, kept by every lane), so that a kernel
   // that loops over several sweeps (loop_sweeps > 1) keeps prefetching across the reduce + LM update between two sweeps.
@@ -473,6 +546,21 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     n_tile = 0;
   };
 
+  // kModeFrames: expands the parked whole frames (one per lane) straight into their report rows -- no warp reduction
+  auto flush_frames = [&]() {
+    __syncwarp();
+    if (lane < n_tile) {
+      const double* row = tile + lane * kTileStride;
+      const double* rx = ftile + lane * 3;
+      const int64_t f = __double_as_longlong(row[12]);
+      const double cost_term = LOSS ? log(row[10]) + row[11] * 0.693147180559945309417232121458 : rx[1];
+      frame_row_write(pv, pc, f, pv.offsets[f + 1] - pv.offsets[f], row, cost_term, rx[0], rx[1], rx[2], LOSS,
+                      args.use_edges && pv.n_edges > 0, args.frame_rows + f * kRowDoubles);
+    }
+    __syncwarp();
+    n_tile = 0;
+  };
+
   int gc_base = 0;
   for (int sw = 0;; ++sw) {  // one pass per sweep (exactly one unless the kernel loops the LM by itself)
   const unsigned int launch_tag = LOOP ? launch_tag0 + (unsigned int)sw : launch_tag0;
@@ -522,12 +610,23 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     Moments a;
     moments_clear<LOSS>(a);
     bool open = false;  // the current piece has accumulated points
+    FrameSums fx;       // kModeFrames only
+    frame_sums_clear(fx);
+    int64_t piece_n = 0;  // kModeFrames: points of the current piece
 
     // sums the lanes' moments of the finished piece and parks them in the tile
     auto park_piece = [&]() {
       double v[16] = {a.S0, a.Sx, a.Sy, a.Sz, a.Sxx, a.Sxy, a.Sxz, a.Syy, a.Syz, a.Szz, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       double pr = a.prod;
       int es = a.esum;
+      double em = 0.0;
+      if (MODE == kModeFrames) {
+        v[12] = fx.se;
+        v[13] = fx.se2;
+        em = fx.emax;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) em = nan_max(em, __shfl_xor_sync(0xffffffffu, em, o));
+      }
       if (LOSS) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
@@ -538,17 +637,41 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         v[10] = pr;  // sum of e^2
       }
       warp_transpose_sum<16>(v, lane);  // lane L: total of moment (L mod 16)
-      {
-        double* row = tile + n_tile * kTileStride;
-        if (lane < 10 || (!LOSS && lane == 10)) row[lane] = v[0];
-        if (LOSS && lane == 10) row[10] = pr;
-        if (lane == 11) row[11] = (double)es;
-        if (lane == 12) row[12] = __longlong_as_double(f);
+      const int kind = MODE == kModeFrames ? frame_piece_kind(pv.offsets[f], f_end, p0, p1) : (int)kPieceWhole;
+      if (kind != kPieceWhole) {
+        // kModeFrames: a piece of a frame that crosses a range end -> this warp's head or tail slot, raw (clc_frames.cuh)
+        double* slot = args.frame_slots + (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kSlotDoubles;
+        if (lane < 10 || lane == 12 || lane == 13) slot[lane] = v[0];
+        if (lane == 10) slot[10] = LOSS ? pr : 0.0;
+        if (lane == 11) slot[11] = (double)es;
+        if (lane == 14) slot[14] = em;
+        if (lane == 15) slot[15] = (double)piece_n;
+      } else {
+        {
+          double* row = tile + n_tile * kTileStride;
+          if (lane < 10 || (!LOSS && lane == 10)) row[lane] = v[0];
+          if (LOSS && lane == 10) row[10] = pr;
+          if (lane == 11) row[11] = (double)es;
+          if (lane == 12) row[12] = __longlong_as_double(f);
+        }
+        if (MODE == kModeFrames) {
+          double* rx = ftile + n_tile * 3;
+          if (lane == 12) rx[0] = v[0];
+          if (lane == 13) rx[1] = v[0];
+          if (lane == 14) rx[2] = em;
+        }
+        ++n_tile;
+        if (n_tile == 32) {
+          if (MODE == kModeFrames) flush_frames();
+          else flush_tile();
+        }
       }
-      ++n_tile;
-      if (n_tile == 32) flush_tile();
       moments_clear<LOSS>(a);
       open = false;
+      if (MODE == kModeFrames) {
+        frame_sums_clear(fx);
+        piece_n = 0;
+      }
     };
 
     for (int ch = 0; ch < n_chunks; ++ch) {
@@ -592,18 +715,23 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         if (q == cb && hi == cb + CH) {
           // the whole stage belongs to one frame: no masks
 #pragma unroll
-          for (int g = 0; g < G; ++g)
+          for (int g = 0; g < G; ++g) {
             process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2);
+            if (MODE == kModeFrames) frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], true, true, m0, m1, m2, c);
+          }
         } else {
 #pragma unroll
           for (int g = 0; g < G; ++g) {
             const int64_t i0 = cb + 64 * g + 2 * lane;
             process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2,
                                             c, pv.inv_a2);
+            if (MODE == kModeFrames)
+              frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2, c);
           }
         }
         if (LOSS) renormalise(a);
         open = true;
+        if (MODE == kModeFrames) piece_n += hi - q;
         q = hi;
         if (hi == f_end) park_piece();
       }
@@ -614,6 +742,11 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       if (kLockstepSlack > 0 && lane == 0) *(volatile int*)&s_prog[warp] = (ch + 1 == n_chunks) ? 0x7fffffff : ch + 1;
     }
     if (open) park_piece();  // the last frame continues in the next warp's range
+  }
+  if (MODE == kModeFrames) {
+    // the rows of whole frames are written; split frames are finished by clc_frame_fixup_kernel -- no block reduction
+    flush_frames();
+    return;
   }
   CLC_STAMP(1);
   if (args.timing != nullptr && lane == 0) args.timing[(int64_t)gridDim.x * 8 + gwarp] = globaltimer_ns();
@@ -860,6 +993,42 @@ __global__ void clc_lm_kernel(LmState* lm, const double* sums) {
     for (int k = 0; k < kNumSums; ++k) s[k] = sums[k];
     lm_update(&lm->core, lm->trace, s);
   }
+}
+
+// ---- K1 fix-up of the per-frame report (after a kModeFrames sweep) ---------------------------------------------------
+// One thread per frame: an empty frame gets a row of zeros; a split frame (clc_frames.cuh) adds the tail slot of its first warp
+// and the head slots of the following warps, in warp order (the row is bit-reproducible), and expands them into its row; the
+// rows of the other frames were written by the sweep.
+template <bool LOSS>
+__global__ void clc_frame_fixup_kernel(ProblemView pv, const double* pose7, int edges, const double* __restrict__ slots,
+                                       double* __restrict__ rows) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= pv.n_frames) return;
+  const int64_t fs = pv.offsets[f], fe = pv.offsets[f + 1];
+  double* row = rows + f * kRowDoubles;
+  if (fe <= fs) {
+    for (int k = 0; k < kRowDoubles; ++k) row[k] = 0.0;
+    return;
+  }
+  int64_t w0, w1;
+  frame_warps(fs, fe, pv.per_warp, &w0, &w1);
+  if (w0 == w1) return;
+  double S[10] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  double cost_term = 0.0, se = 0.0, se2 = 0.0, emax = 0.0;
+  int64_t n = 0;
+  for (int64_t w = w0; w <= w1; ++w) {
+    const double* s = slots + frame_slot(w, w0);
+#pragma unroll
+    for (int k = 0; k < 10; ++k) S[k] += s[k];
+    cost_term += LOSS ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[13];
+    se += s[12];
+    se2 += s[13];
+    emax = nan_max(emax, s[14]);
+    n += (int64_t)s[15];
+  }
+  PoseConsts pc;
+  make_pose_consts(pose7, &pc);
+  frame_row_write(pv, pc, f, n, S, cost_term, se, se2, emax, LOSS, edges != 0, row);
 }
 
 // ---- K0: layout kernels ------------------------------------------------------------------------------------------

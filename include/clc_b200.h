@@ -190,6 +190,24 @@ int clc_solve_lm(clc_problem* p, double pose7[7], const clc_lm_options* opt, clc
 int clc_information(clc_problem* p, const double pose7[7], double H36[36], double b6[6], double* chi,
                     double singular_values6[6], double V36[36]);
 
+/* Per-frame report: every frame's residual statistics and its share of the normal equations, from ONE streaming sweep of the
+ * device-resident problem at pose7 -- which frames drive the result, and which ones disagree with it.  Summed over the frames,
+ * `cost` gives clc_eval's cost, H21 and g6 give clc_eval's H and g (upper triangle, K1's order), and `chi` gives
+ * clc_information's chi, at the same pose (up to the order of summation).  With H and g of clc_eval, -(H - H_f)^-1 (g - g_f)
+ * is a one-step estimate of how far the extrinsic moves without frame f (camlasercalibratool_b200.frame_influence). */
+typedef struct {
+  int64_t n_points;        /* points of the frame (0: empty frame, every other field 0) */
+  double cost;             /* 1/2 sum rho over the frame's residuals (points + its edge residuals), the Cauchy loss as the problem has it */
+  double chi;              /* s^2 sum e^2 over the points, no loss, no edges: the frame's share of clc_information's chi */
+  double mean_e, rms_e, max_abs_e; /* metres, over the points, unweighted (max_abs_e is NaN when a point's distance is NaN) */
+  double mean_weight;      /* sum w / n (1 without loss) */
+  double edge_e[2];        /* raw residuals of the two edge residuals (0 without edges) */
+  double H21[21], g6[6];   /* the frame's share of clc_eval's H (upper triangle, K1's order) and g */
+} clc_frame_row;
+/* rows[n_frames] (host memory the caller sizes: 288 bytes per frame), copied from the device once.  A problem attached to a
+ * communicator reports its own frames (its clc_shard_range); no collective. */
+int clc_frame_report(clc_problem* p, const double pose7[7], clc_frame_row* rows);
+
 /* replaces: CamLaserCalClosedSolution(), reference src/LaseCamCalCeres.cpp:112-203.  Tlc16 row-major.
  * AtA81/Atb9 (the 9x9 normal equations) may be NULL. */
 int clc_closed_form(clc_problem* p, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
@@ -276,6 +294,8 @@ int clc_group_solve_lm(clc_group* g, double pose7[7], const clc_lm_options* opt,
 int clc_group_information(clc_group* g, const double pose7[7], double H36[36], double b6[6], double* chi,
                           double singular_values6[6], double V36[36]);
 int clc_group_closed_form(clc_group* g, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
+/* clc_frame_report of every shard: rows[all frames of the group], in the global frame order */
+int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* rows);
 /* The device list the reference-facing drop-in uses (its signatures have no device argument): environment variable
  * CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device only).  Writes at most `cap` ordinals. */
 int clc_default_devices(int* devices, int cap, int* n);
@@ -285,6 +305,9 @@ int clc_default_devices(int* devices, int cap, int* n);
  * flush_l2 != 0 overwrites a buffer larger than L2 between launches (outside the timed brackets).
  * ms_each[n] receives the per-launch device times.  No collective, local shard only. */
 int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each);
+/* The same for clc_frame_report: each bracket holds the per-frame sweep and the split-frame fix-up, not the copy of the rows
+ * to the host. */
+int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each);
 /* Algorithmic bytes of one K1 launch on this problem: 24*P + 40*N + 56*edges + 224 (SURVEY.md section 8(d)). */
 int clc_problem_algorithmic_bytes(const clc_problem* p, int64_t* bytes);
 /* Bytes one K1 launch actually streams: the figure above with 16 instead of 24 bytes per point when the planar
