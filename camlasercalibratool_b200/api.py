@@ -160,6 +160,16 @@ def frame_influence(report, H, g):
     return delta, np.linalg.norm(delta[:, :3], axis=1), np.linalg.norm(delta[:, 3:], axis=1)
 
 
+def _keep_mask(keep, n_frames):
+    """A boolean mask of length n_frames -> the uint8 array of the C ABI (checked before any device work)."""
+    keep = np.asarray(keep)
+    if keep.dtype != np.bool_:
+        raise TypeError(f"keep must be a boolean mask, not {keep.dtype}")
+    if keep.shape != (n_frames,):
+        raise ValueError(f"keep must have shape ({n_frames},), not {keep.shape}")
+    return np.ascontiguousarray(keep, dtype=np.uint8)
+
+
 def default_options(**kw) -> LmOptions:
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
@@ -223,6 +233,16 @@ class Problem:
         h = C.c_void_p()
         _lib.check(L.clc_problem_create_synthetic(C.byref(h), C.byref(d)), "clc_problem_create_synthetic")
         return cls(h)
+
+    def subset(self, keep):
+        """A new problem of the frames with keep[f] True, in their order (clc_problem_subset), built on the device from this
+        one's data -- no upload.  It is the problem from_arrays would build from the kept frames, so every output is bit-identical
+        to that fresh problem's.  This problem is unchanged; close it when it is no longer needed.  While both are alive the
+        device holds the kept share a second time."""
+        k = _keep_mask(keep, self.sizes()[0])
+        h = C.c_void_p()
+        _lib.check(self._L.clc_problem_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(h)), "clc_problem_subset")
+        return Problem(h)
 
     def close(self):
         if self._h is not None:
@@ -375,6 +395,14 @@ class Problem:
         _lib.check(self._L.clc_bench_frame_report(self._h, _dp(pose7), int(n), int(bool(flush_l2)), ms), "clc_bench_frame_report")
         return np.array(ms[:], dtype=np.float64)
 
+    def bench_subset(self, keep, n, flush_l2=True):
+        """Device time of the gather of n subsets(keep) into scratch problems (clc_bench_subset), ms each."""
+        k = _keep_mask(keep, self.sizes()[0])
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), int(n), int(bool(flush_l2)), ms),
+                   "clc_bench_subset")
+        return np.array(ms[:], dtype=np.float64)
+
 
 class Group:
     """G devices of THIS process solving one problem (clc_group_*): frames sharded by point count, the 28 sums exchanged
@@ -415,6 +443,15 @@ class Group:
         h = C.c_void_p()
         _lib.check(_lib.load().clc_group_create_synthetic(C.byref(h), C.byref(d), arr, n), "clc_group_create_synthetic")
         return cls(h)
+
+    def subset(self, keep):
+        """Problem.subset for the group (clc_group_subset): a new group on the same devices holding the frames with keep[f]
+        True, re-sharded as from_frames would shard them; kept points on another device are copied over the peer links.  This
+        group is unchanged; close it when it is no longer needed."""
+        k = _keep_mask(keep, self.sizes()[1])
+        h = C.c_void_p()
+        _lib.check(self._L.clc_group_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(h)), "clc_group_subset")
+        return Group(h)
 
     def close(self):
         if self._h is not None:

@@ -24,6 +24,8 @@
 #include "clc_l2_plan.h"
 #include "clc_linefit.cuh"
 #include "clc_small.cuh"
+#include "clc_subset.cuh"
+#include "clc_subset_plan.h"
 
 namespace {
 
@@ -1710,17 +1712,8 @@ int clc_shard_range(int64_t n_frames, const int64_t* offsets, int nranks, int ra
     *end = n_frames * (rank + 1) / nranks;
     return CLC_OK;
   }
-  // contiguous ranges balanced by point count: boundary r is the first frame whose start >= r * P / nranks
-  const int64_t P = offsets[n_frames];
-  auto boundary = [&](int r) -> int64_t {
-    if (r <= 0) return 0;
-    if (r >= nranks) return n_frames;
-    const int64_t target = (int64_t)((__int128)P * r / nranks);
-    return std::lower_bound(offsets, offsets + n_frames + 1, target) - offsets;
-  };
-  *begin = boundary(rank);
-  *end = boundary(rank + 1);
-  if (*end < *begin) *end = *begin;
+  // contiguous ranges balanced by point count (clc_subset_plan.h, which re-shards a group's subset the same way)
+  clc::balanced_shard_range(n_frames, offsets, nranks, rank, begin, end);
   return CLC_OK;
 }
 
@@ -2126,6 +2119,306 @@ int clc_group_solve_lm(clc_group* g, double pose7[7], const clc_lm_options* opt,
   return solve_all(g->problems.data(), (int)g->problems.size(), pose7, opt, summary, trace, trace_cap);
 }
 
+// ---- subsets: a new problem from the kept frames of a device-resident one (clc_subset_plan.h, clc_subset.cuh) ---------------
+
+namespace {
+
+int check_keep(int64_t n_frames, const uint8_t* keep) {
+  for (int64_t f = 0; f < n_frames; ++f)
+    if (keep[f] > 1) return fail(CLC_ERR_INVALID, "keep[" + std::to_string(f) + "] is neither 0 nor 1");
+  return CLC_OK;
+}
+
+// One destination shard of a subset while it is being built: the shell, and the gather's inputs in one device buffer
+// (runs [n_runs * 4] | first run of every tile [n_tiles] | source of every frame [n_frames]).
+struct SubsetShard {
+  clc_problem* p = nullptr;
+  int64_t* d_work = nullptr;
+  clc::SubsetArgs args = {};
+  bool gathers_z = false;  // some kept point comes from a source whose z is not known to be all 0
+};
+
+void subset_release(std::vector<SubsetShard>& shards) {
+  for (SubsetShard& s : shards) {
+    if (!s.p) continue;
+    if (s.d_work && cudaSetDevice(s.p->device) == cudaSuccess) cudaFreeAsync(s.d_work, s.p->stream);
+    clc_problem_destroy(s.p);
+  }
+  shards.clear();
+}
+
+// The shell of a destination shard: sizes, the source's loss, point arrays with zeroed padding, per-frame arrays, offsets.
+int subset_shell(clc_problem** out, int device, int64_t N, int64_t P, const int64_t* offsets, bool with_z, bool edges,
+                 bool true_poses, int use_loss, double cauchy_a) {
+  clc_problem* p = new clc_problem();
+  *out = p;
+  int rc = init_device(p, device);
+  if (rc != CLC_OK) return rc;
+  p->n_frames = N;
+  p->n_points = P;
+  p->n_edges = edges ? 2 * N : 0;
+  p->use_loss = use_loss;
+  p->cauchy_a = cauchy_a;
+  rc = alloc_points(p, with_z);
+  if (rc != CLC_OK) return rc;
+  CLC_CUDA(cudaMallocAsync(&p->frame_pose, sizeof(double) * 7 * std::max<int64_t>(N, 1), p->stream));
+  CLC_CUDA(cudaMallocAsync(&p->plane, sizeof(double) * 4 * std::max<int64_t>(N, 1), p->stream));
+  CLC_CUDA(cudaMallocAsync(&p->offsets, sizeof(int64_t) * (N + 1), p->stream));
+  CLC_CUDA(cudaMemcpyAsync(p->offsets, offsets, sizeof(int64_t) * (N + 1), cudaMemcpyHostToDevice, p->stream));
+  if (p->n_edges > 0) {
+    CLC_CUDA(cudaMallocAsync(&p->edge_plane, sizeof(double) * 4 * p->n_edges, p->stream));
+    CLC_CUDA(cudaMallocAsync(&p->edge_pt, sizeof(double) * 3 * p->n_edges, p->stream));
+  }
+  if (true_poses) CLC_CUDA(cudaMallocAsync(&p->frame_pose_true, sizeof(double) * 7 * std::max<int64_t>(N, 1), p->stream));
+  return CLC_OK;
+}
+
+// Plans the subset of the source shards `src` (in frame order) and builds the shells of its destination shards, one per
+// entry of `devices`, with the gather's inputs uploaded.  Only the source offsets come to the host.
+int subset_prepare(const std::vector<clc_problem*>& src, const uint8_t* keep, const std::vector<int>& devices,
+                   std::vector<SubsetShard>* out) {
+  const int S = (int)src.size(), G = (int)devices.size();
+  if (S > clc::kMaxRanks) return fail(CLC_ERR_INVALID, "too many source shards");
+  std::vector<std::vector<int64_t>> src_off((size_t)S);
+  std::vector<const int64_t*> off_ptr((size_t)S);
+  std::vector<int64_t> src_frames((size_t)S);
+  clc::SubsetArgs base = {};
+  bool edges = false;
+  for (int s = 0; s < S; ++s) {
+    const clc_problem* q = src[s];
+    CLC_CUDA(cudaSetDevice(q->device));
+    CLC_CUDA(cudaStreamSynchronize(q->stream));  // nothing the caller enqueued may still write the source
+    src_off[s].resize((size_t)q->n_frames + 1);
+    CLC_CUDA(cudaMemcpy(src_off[s].data(), q->offsets, sizeof(int64_t) * (q->n_frames + 1), cudaMemcpyDeviceToHost));
+    off_ptr[s] = src_off[s].data();
+    src_frames[s] = q->n_frames;
+    // the copies below use 16-byte vectors: every coordinate array is allocated 16-byte aligned (alloc_points, alloc_z)
+    if ((reinterpret_cast<uintptr_t>(q->x) | reinterpret_cast<uintptr_t>(q->y) | reinterpret_cast<uintptr_t>(q->z)) & 15)
+      return fail(CLC_ERR_STATE, "internal: misaligned coordinate array");
+    // a z stream that is known to be all 0 (planar data on the general kernels) is not read: the destination writes 0
+    base.src[s] = {q->x, q->y, q->z_all_zero ? nullptr : q->z, q->frame_pose, q->edge_pt, q->frame_pose_true};
+    edges = edges || q->n_edges > 0;
+  }
+  const clc::SubsetPlan plan = clc::subset_plan(S, off_ptr.data(), src_frames.data(), keep, G);
+  const bool true_poses = src[0]->frame_pose_true != nullptr;
+  out->assign((size_t)G, SubsetShard());
+  size_t seg = 0;
+  for (int d = 0; d < G; ++d) {
+    SubsetShard& sh = (*out)[d];
+    const int64_t fb = plan.shard_frame[d], fe = plan.shard_frame[d + 1], N = fe - fb;
+    const int64_t P = plan.offsets[fe] - plan.offsets[fb];
+    std::vector<int64_t> offsets((size_t)N + 1);
+    for (int64_t f = 0; f <= N; ++f) offsets[f] = plan.offsets[fb + f] - plan.offsets[fb];
+    // runs with points, the first run of every tile, the source of every frame
+    std::vector<int64_t> runs, frame_src((size_t)N);
+    for (; seg < plan.segments.size() && plan.segments[seg].dst_shard == d; ++seg) {
+      const clc::SubsetSegment& c = plan.segments[seg];
+      for (int64_t k = 0; k < c.n_frames; ++k)
+        frame_src[c.dst_frame + k] = ((int64_t)c.src_shard << clc::kSubsetShardShift) + c.src_frame + k;
+      if (c.n_points == 0) continue;
+      runs.insert(runs.end(), {(int64_t)c.src_shard, c.src_point, c.dst_point, c.n_points});
+      sh.gathers_z = sh.gathers_z || base.src[c.src_shard].z != nullptr;
+    }
+    const int64_t n_runs = (int64_t)runs.size() / 4, n_tiles = (P + clc::kSubsetTile - 1) / clc::kSubsetTile;
+    std::vector<int64_t> work(runs);
+    for (int64_t t = 0, r = 0; t < n_tiles; ++t) {
+      while (runs[4 * r + 2] + runs[4 * r + 3] <= t * clc::kSubsetTile) ++r;  // runs cover [0, P) without gaps
+      work.push_back(r);
+    }
+    work.insert(work.end(), frame_src.begin(), frame_src.end());
+    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]->use_loss,
+                          src[0]->cauchy_a);
+    if (rc != CLC_OK) return rc;
+    clc_problem* p = sh.p;
+    CLC_CUDA(cudaMallocAsync(&sh.d_work, sizeof(int64_t) * std::max<size_t>(work.size(), 1), p->stream));
+    if (!work.empty())
+      CLC_CUDA(cudaMemcpyAsync(sh.d_work, work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
+    clc::SubsetArgs& a = sh.args;
+    a = base;
+    a.runs = sh.d_work;
+    a.tile_run = sh.d_work + 4 * n_runs;
+    a.frame_src = sh.d_work + 4 * n_runs + n_tiles;
+    a.n_runs = n_runs;
+    a.n_tiles = n_tiles;
+    a.n_frames = N;
+    a.x = p->x;
+    a.y = p->y;
+    a.z = p->z;
+    a.frame_pose = p->frame_pose;
+    a.edge_pt = p->edge_pt;
+    a.frame_pose_true = p->frame_pose_true;
+    a.nonplanar = p->d_nonplanar;
+    // pageable host memory: the copies above have been staged when they return, the host vectors may go
+  }
+  return CLC_OK;
+}
+
+int subset_launch(const SubsetShard& sh, cudaStream_t stream) {
+  const clc::SubsetArgs& a = sh.args;
+  const int64_t blocks = a.n_tiles + (a.n_frames + clc::kSubsetThreads - 1) / clc::kSubsetThreads;
+  if (blocks == 0) return CLC_OK;
+  clc::clc_subset_gather_kernel<<<(unsigned)blocks, clc::kSubsetThreads, 0, stream>>>(a);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// After the gather: the planarity verdict, then the creation tail every problem goes through.  A gathered z stream that
+// holds only zeros is dropped first, so that the problem is the one a fresh creation from the kept frames builds (the host
+// packers never create the z stream of all-zero data; finish_create materialises +0.0 zeros if the general kernels need them).
+int subset_finish(SubsetShard& sh) {
+  clc_problem* p = sh.p;
+  CLC_CUDA(cudaSetDevice(p->device));
+  p->host_planarity_known = true;
+  p->z_all_zero = true;
+  if (sh.gathers_z) {
+    int nonplanar = 1;
+    CLC_CUDA(cudaMemcpyAsync(&nonplanar, p->d_nonplanar, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
+    p->z_all_zero = nonplanar == 0;
+    if (p->z_all_zero) {
+      CLC_CUDA(cudaFreeAsync(p->z_block, p->stream));
+      p->z = nullptr;
+      p->z_block = nullptr;
+    }
+  }
+  CLC_CUDA(cudaFreeAsync(sh.d_work, p->stream));
+  sh.d_work = nullptr;
+  return finish_create(p);
+}
+
+// Cross-device reads of a group's subset.  The points and per-frame arrays live in each device's default memory pool
+// (cudaMallocAsync), and pool memory does not follow cudaDeviceEnablePeerAccess: another device may read it only once the pool
+// grants that device access (cudaMemPoolSetAccess).  The gather opens every source device's pool to every other destination
+// device that lacks access, and closes it again once the gathers are complete -- a subset leaves the pools as it found them.
+// One gather at a time in the process may hold such grants.
+std::mutex g_pool_grant_mutex;
+
+struct PoolGrant {
+  cudaMemPool_t pool;
+  int device;  // the device that was given access
+};
+
+int pool_access_set(const std::vector<PoolGrant>& grants, cudaMemAccessFlags flags) {
+  for (const PoolGrant& g : grants) {
+    cudaMemAccessDesc desc = {};
+    desc.location.type = cudaMemLocationTypeDevice;
+    desc.location.id = g.device;
+    desc.flags = flags;
+    CLC_CUDA(cudaMemPoolSetAccess(g.pool, &desc, 1));
+  }
+  return CLC_OK;
+}
+
+int pool_access_open(const std::vector<clc_problem*>& src, const std::vector<int>& devices, std::vector<PoolGrant>* grants) {
+  std::vector<int> owners;
+  for (const clc_problem* q : src)
+    if (std::find(owners.begin(), owners.end(), q->device) == owners.end()) owners.push_back(q->device);
+  for (int owner : owners) {
+    cudaMemPool_t pool;
+    CLC_CUDA(cudaDeviceGetDefaultMemPool(&pool, owner));
+    for (size_t i = 0; i < devices.size(); ++i) {
+      const int d = devices[i];
+      if (d == owner || std::find(devices.begin(), devices.begin() + (long)i, d) != devices.begin() + (long)i) continue;
+      cudaMemLocation loc = {};
+      loc.type = cudaMemLocationTypeDevice;
+      loc.id = d;
+      cudaMemAccessFlags have = cudaMemAccessFlagsProtNone;
+      CLC_CUDA(cudaMemPoolGetAccess(&have, pool, &loc));
+      if (have == cudaMemAccessFlagsProtReadWrite) continue;  // granted by the caller: theirs to keep
+      grants->push_back({pool, d});
+      int rc = pool_access_set({grants->back()}, cudaMemAccessFlagsProtReadWrite);
+      if (rc != CLC_OK) {
+        grants->pop_back();
+        return rc;
+      }
+    }
+  }
+  return CLC_OK;
+}
+
+// the whole subset: plan, shells, one gather per destination shard (all devices in flight), finish
+int subset_build(const std::vector<clc_problem*>& src, const uint8_t* keep, const std::vector<int>& devices,
+                 std::vector<clc_problem*>* out) {
+  std::vector<SubsetShard> shards;
+  int rc = subset_prepare(src, keep, devices, &shards);
+  bool cross_device = false;
+  for (const clc_problem* q : src)
+    for (int d : devices) cross_device = cross_device || d != q->device;
+  std::unique_lock<std::mutex> grant_lock(g_pool_grant_mutex, std::defer_lock);
+  std::vector<PoolGrant> grants;
+  if (rc == CLC_OK && cross_device) {
+    grant_lock.lock();
+    rc = pool_access_open(src, devices, &grants);
+  }
+  for (size_t d = 0; d < shards.size() && rc == CLC_OK; ++d) {
+    rc = set_device(shards[d].p);
+    if (rc == CLC_OK) rc = subset_launch(shards[d], shards[d].p->stream);
+  }
+  if (!grants.empty()) {
+    // every gather has to be complete before another device's access goes away
+    for (SubsetShard& sh : shards)
+      if (sh.p && sh.p->stream && cudaSetDevice(sh.p->device) == cudaSuccess) {
+        const cudaError_t e = cudaStreamSynchronize(sh.p->stream);
+        if (e != cudaSuccess && rc == CLC_OK) rc = fail(CLC_ERR_CUDA, std::string("subset gather: ") + cudaGetErrorString(e));
+      }
+    const std::string msg = g_last_error;
+    const int rc_close = pool_access_set(grants, cudaMemAccessFlagsProtNone);
+    if (rc == CLC_OK) rc = rc_close;
+    else g_last_error = msg;
+  }
+  if (grant_lock.owns_lock()) grant_lock.unlock();
+  for (size_t d = 0; d < shards.size() && rc == CLC_OK; ++d) rc = subset_finish(shards[d]);
+  if (rc != CLC_OK) {
+    const std::string msg = g_last_error;
+    subset_release(shards);
+    g_last_error = msg;
+    return rc;
+  }
+  for (SubsetShard& s : shards) out->push_back(s.p);
+  return CLC_OK;
+}
+
+}  // namespace
+
+int clc_problem_subset(const clc_problem* src, const uint8_t* keep, clc_problem** out) {
+  if (!src || !keep || !out) return fail(CLC_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  int rc = check_keep(src->n_frames, keep);
+  if (rc != CLC_OK) return rc;
+  std::vector<clc_problem*> ps;
+  rc = subset_build({const_cast<clc_problem*>(src)}, keep, {src->device}, &ps);
+  if (rc != CLC_OK) return rc;
+  *out = ps[0];
+  return CLC_OK;
+}
+
+int clc_group_subset(const clc_group* src, const uint8_t* keep, clc_group** out) {
+  if (!src || !keep || !out) return fail(CLC_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  if (src->problems.empty()) return fail(CLC_ERR_INVALID, "empty group");
+  int rc = check_keep(src->n_frames, keep);
+  if (rc != CLC_OK) return rc;
+  std::vector<int> devs;
+  for (const clc_problem* p : src->problems) devs.push_back(p->device);
+  clc_group* g = new clc_group();
+  rc = subset_build(src->problems, keep, devs, &g->problems);
+  if (rc == CLC_OK) {
+    for (const clc_problem* p : g->problems) {
+      g->n_frames += p->n_frames;
+      g->n_points += p->n_points;
+    }
+    rc = group_attach(g, devs.data(), (int)devs.size());
+  }
+  if (rc != CLC_OK) {
+    const std::string msg = g_last_error;
+    clc_group_destroy(g);
+    g_last_error = msg;
+    return rc;
+  }
+  *out = g;
+  return CLC_OK;
+}
+
 // Devices the reference-facing drop-in uses (its signatures have no device argument): the environment variable
 // CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device).
 int clc_default_devices(int* devices, int cap, int* n) {
@@ -2311,6 +2604,29 @@ int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flu
   rc = frame_report_alloc(p, &b);
   if (rc == CLC_OK) rc = bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return frame_report_launch(p, b); });
   frame_report_free(p, &b);
+  return rc;
+}
+
+int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2, float* ms_each) {
+  if (!src || !keep || n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_keep(src->n_frames, keep);
+  if (rc != CLC_OK) return rc;
+  clc_problem* p = src;
+  rc = set_device(p);
+  int flush_smem = 0;
+  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
+  for (int i = 0; i < n && rc == CLC_OK; ++i) {
+    // a fresh scratch problem every time; its gather runs on the source's stream, behind the source's L2 flush
+    std::vector<SubsetShard> shards;
+    rc = subset_prepare({p}, keep, {p->device}, &shards);
+    if (rc == CLC_OK) rc = shards[0].p->stream && cudaStreamSynchronize(shards[0].p->stream) == cudaSuccess
+                                ? CLC_OK : fail(CLC_ERR_CUDA, "scratch problem");
+    if (rc == CLC_OK) rc = set_device(p);
+    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &ms_each[i], [&]() { return subset_launch(shards[0], p->stream); });
+    const std::string msg = g_last_error;
+    subset_release(shards);
+    g_last_error = msg;
+  }
   return rc;
 }
 

@@ -296,6 +296,23 @@ int clc_group_information(clc_group* g, const double pose7[7], double H36[36], d
 int clc_group_closed_form(clc_group* g, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
 /* clc_frame_report of every shard: rows[all frames of the group], in the global frame order */
 int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* rows);
+/* ---- subsets: solve again without some frames, without sending the points through the host again -----------------------
+ * A new problem on src's device holding only the frames with keep[f] == 1 (keep has src's n_frames entries, each 0 or 1), in
+ * their original order, built from src's device-resident data: only src's frame offsets come to the host, a gather kernel copies
+ * the kept points and per-frame arrays.  The result is the problem clc_problem_create would build from the kept frames' poses,
+ * points and edge points -- the same layout, planes, planarity verdict, kernel family, partition and dispatch, so every output is
+ * bit-identical to that fresh problem's.  (One exception in the stored bytes: the sign of a z that is -0.0 or +0.0.  A fresh upload
+ * stores such a z as +0.0 or as given depending on whether a z != 0 shares its upload chunk; the subset copies it as the source
+ * holds it, or writes +0.0 where the source has no z stream.  Both signs give the same results.)  It inherits use_loss, cauchy_a and (synthetic camera-mode sources) the true poses; it
+ * starts in the default planar mode and is attached to no communicator.  src is unchanged and stays valid; both need device
+ * memory at once.  Keeping every frame or none is valid.  A NULL argument or a keep entry other than 0 or 1 fails with
+ * CLC_ERR_INVALID before the device is touched. */
+int clc_problem_subset(const clc_problem* src, const uint8_t* keep, clc_problem** out);
+/* The same for an in-process group: a new group on the same device list, the kept frames re-sharded over it as
+ * clc_group_create_gather shards a fresh problem.  Kept points on another device are read over the peer links: for the gather,
+ * each source device's default memory pool is opened to the other devices of the group (cudaMemPoolSetAccess) and closed again
+ * afterwards, unless the caller had already granted that access. */
+int clc_group_subset(const clc_group* src, const uint8_t* keep, clc_group** out);
 /* The device list the reference-facing drop-in uses (its signatures have no device argument): environment variable
  * CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device only).  Writes at most `cap` ordinals. */
 int clc_default_devices(int* devices, int cap, int* n);
@@ -308,6 +325,10 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
 /* The same for clc_frame_report: each bracket holds the per-frame sweep and the split-frame fix-up, not the copy of the rows
  * to the host. */
 int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each);
+/* The gather of clc_problem_subset(src, keep): `n` times a scratch subset is prepared, its gather kernel is timed alone (CUDA
+ * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
+ * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
+int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2, float* ms_each);
 /* Algorithmic bytes of one K1 launch on this problem: 24*P + 40*N + 56*edges + 224 (SURVEY.md section 8(d)). */
 int clc_problem_algorithmic_bytes(const clc_problem* p, int64_t* bytes);
 /* Bytes one K1 launch actually streams: the figure above with 16 instead of 24 bytes per point when the planar
