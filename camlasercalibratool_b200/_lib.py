@@ -176,6 +176,8 @@ SIGNATURES = {
     "clc_group_frame_report": (C.c_int, [_P, c_double_p, _P]),
     "clc_problem_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.POINTER(_P)]),
     "clc_group_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.POINTER(_P)]),
+    "clc_problem_trim": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(_P)]),
+    "clc_group_trim": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(_P)]),
     "clc_default_devices": (C.c_int, [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     "clc_upload_last_stats": (C.c_int, [c_double_p, c_double_p, c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "clc_problem_destroy": (C.c_int, [_P]),
@@ -206,6 +208,7 @@ SIGNATURES = {
     "clc_bench_eval": (C.c_int, [_P, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_frame_report": (C.c_int, [_P, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.POINTER(C.c_float)]),
+    "clc_bench_trim": (C.c_int, [_P, c_double_p, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "clc_problem_algorithmic_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_streamed_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_set_planar_mode": (C.c_int, [_P, C.c_int]),

@@ -170,6 +170,19 @@ def _keep_mask(keep, n_frames):
     return np.ascontiguousarray(keep, dtype=np.uint8)
 
 
+def _thresholds(max_abs_e, n_frames):
+    """A scalar (every frame) or an array of shape (n_frames,) -> the float64 thresholds of the C ABI (checked before any
+    device work: the library rejects a NaN or negative entry too)."""
+    t = np.asarray(max_abs_e, dtype=np.float64)
+    if t.ndim == 0:
+        t = np.full(n_frames, float(t))
+    elif t.shape != (n_frames,):
+        raise ValueError(f"max_abs_e must be a scalar or have shape ({n_frames},), not {t.shape}")
+    if np.any(~(t >= 0.0)):
+        raise ValueError("max_abs_e must not be NaN or negative")
+    return np.ascontiguousarray(t)
+
+
 def default_options(**kw) -> LmOptions:
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
@@ -242,6 +255,18 @@ class Problem:
         k = _keep_mask(keep, self.sizes()[0])
         h = C.c_void_p()
         _lib.check(self._L.clc_problem_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(h)), "clc_problem_subset")
+        return Problem(h)
+
+    def trim(self, pose7, max_abs_e):
+        """A new problem without the points farther than max_abs_e[f] from their board at pose7 (clc_problem_trim), built on the
+        device from this one's data -- no upload.  max_abs_e: a scalar for every frame or one threshold per frame, in the units
+        of frame_report's max_abs_e (e.g. 3 * frame_report(x)["rms_e"]); points whose distance is NaN are always dropped.  Every
+        frame stays, possibly empty.  It is the problem from_arrays would build from the kept points, so every output is
+        bit-identical to that fresh problem's.  This problem is unchanged; close it when it is no longer needed."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        t = _thresholds(max_abs_e, self.sizes()[0])
+        h = C.c_void_p()
+        _lib.check(self._L.clc_problem_trim(self._h, _dp(pose7), _dp(t), C.byref(h)), "clc_problem_trim")
         return Problem(h)
 
     def close(self):
@@ -403,6 +428,15 @@ class Problem:
                    "clc_bench_subset")
         return np.array(ms[:], dtype=np.float64)
 
+    def bench_trim(self, pose7, max_abs_e, n, flush_l2=True):
+        """Device times of the mark and the gather pass of n trims(pose7, max_abs_e) into scratch problems (clc_bench_trim),
+        ms each: returns (mark [n], gather [n])."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        t = _thresholds(max_abs_e, self.sizes()[0])
+        mark, gather = (C.c_float * n)(), (C.c_float * n)()
+        _lib.check(self._L.clc_bench_trim(self._h, _dp(pose7), _dp(t), int(n), int(bool(flush_l2)), mark, gather), "clc_bench_trim")
+        return np.array(mark[:], dtype=np.float64), np.array(gather[:], dtype=np.float64)
+
 
 class Group:
     """G devices of THIS process solving one problem (clc_group_*): frames sharded by point count, the 28 sums exchanged
@@ -451,6 +485,16 @@ class Group:
         k = _keep_mask(keep, self.sizes()[1])
         h = C.c_void_p()
         _lib.check(self._L.clc_group_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(h)), "clc_group_subset")
+        return Group(h)
+
+    def trim(self, pose7, max_abs_e):
+        """Problem.trim for the group (clc_group_trim), max_abs_e per frame in the global frame order: a new group on the same
+        devices, its frames re-sharded by their new point counts as from_frames would shard them; kept points on another device
+        are copied over the peer links.  This group is unchanged; close it when it is no longer needed."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        t = _thresholds(max_abs_e, self.sizes()[1])
+        h = C.c_void_p()
+        _lib.check(self._L.clc_group_trim(self._h, _dp(pose7), _dp(t), C.byref(h)), "clc_group_trim")
         return Group(h)
 
     def close(self):

@@ -10,6 +10,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <cstddef>
 #include <cstdio>
 #include <cstdlib>
@@ -26,6 +27,7 @@
 #include "clc_small.cuh"
 #include "clc_subset.cuh"
 #include "clc_subset_plan.h"
+#include "clc_trim.cuh"
 
 namespace {
 
@@ -2336,37 +2338,41 @@ int pool_access_open(const std::vector<clc_problem*>& src, const std::vector<int
   return CLC_OK;
 }
 
-// the whole subset: plan, shells, one gather per destination shard (all devices in flight), finish
-int subset_build(const std::vector<clc_problem*>& src, const uint8_t* keep, const std::vector<int>& devices,
-                 std::vector<clc_problem*>* out) {
-  std::vector<SubsetShard> shards;
-  int rc = subset_prepare(src, keep, devices, &shards);
+// Launches the gather of every destination shard (launch(d); all devices in flight).  When a shard reads another device's
+// source, every source pool is opened to the destination devices first, and after the gathers are complete it is closed again.
+int gather_shards(const std::vector<clc_problem*>& src, const std::vector<int>& devices, std::vector<SubsetShard>& shards,
+                  const std::function<int(size_t)>& launch) {
   bool cross_device = false;
   for (const clc_problem* q : src)
     for (int d : devices) cross_device = cross_device || d != q->device;
   std::unique_lock<std::mutex> grant_lock(g_pool_grant_mutex, std::defer_lock);
   std::vector<PoolGrant> grants;
-  if (rc == CLC_OK && cross_device) {
+  int rc = CLC_OK;
+  if (cross_device) {
     grant_lock.lock();
     rc = pool_access_open(src, devices, &grants);
   }
   for (size_t d = 0; d < shards.size() && rc == CLC_OK; ++d) {
     rc = set_device(shards[d].p);
-    if (rc == CLC_OK) rc = subset_launch(shards[d], shards[d].p->stream);
+    if (rc == CLC_OK) rc = launch(d);
   }
   if (!grants.empty()) {
     // every gather has to be complete before another device's access goes away
     for (SubsetShard& sh : shards)
       if (sh.p && sh.p->stream && cudaSetDevice(sh.p->device) == cudaSuccess) {
         const cudaError_t e = cudaStreamSynchronize(sh.p->stream);
-        if (e != cudaSuccess && rc == CLC_OK) rc = fail(CLC_ERR_CUDA, std::string("subset gather: ") + cudaGetErrorString(e));
+        if (e != cudaSuccess && rc == CLC_OK) rc = fail(CLC_ERR_CUDA, std::string("gather: ") + cudaGetErrorString(e));
       }
     const std::string msg = g_last_error;
     const int rc_close = pool_access_set(grants, cudaMemAccessFlagsProtNone);
     if (rc == CLC_OK) rc = rc_close;
     else g_last_error = msg;
   }
-  if (grant_lock.owns_lock()) grant_lock.unlock();
+  return rc;
+}
+
+// After the gathers (rc: how far they got): every destination shard's creation tail, or the release of them all on an error.
+int finish_shards(std::vector<SubsetShard>& shards, int rc, std::vector<clc_problem*>* out) {
   for (size_t d = 0; d < shards.size() && rc == CLC_OK; ++d) rc = subset_finish(shards[d]);
   if (rc != CLC_OK) {
     const std::string msg = g_last_error;
@@ -2376,6 +2382,16 @@ int subset_build(const std::vector<clc_problem*>& src, const uint8_t* keep, cons
   }
   for (SubsetShard& s : shards) out->push_back(s.p);
   return CLC_OK;
+}
+
+// the whole subset: plan, shells, one gather per destination shard (all devices in flight), finish
+int subset_build(const std::vector<clc_problem*>& src, const uint8_t* keep, const std::vector<int>& devices,
+                 std::vector<clc_problem*>* out) {
+  std::vector<SubsetShard> shards;
+  int rc = subset_prepare(src, keep, devices, &shards);
+  if (rc == CLC_OK)
+    rc = gather_shards(src, devices, shards, [&](size_t d) { return subset_launch(shards[d], shards[d].p->stream); });
+  return finish_shards(shards, rc, out);
 }
 
 }  // namespace
@@ -2402,6 +2418,219 @@ int clc_group_subset(const clc_group* src, const uint8_t* keep, clc_group** out)
   for (const clc_problem* p : src->problems) devs.push_back(p->device);
   clc_group* g = new clc_group();
   rc = subset_build(src->problems, keep, devs, &g->problems);
+  if (rc == CLC_OK) {
+    for (const clc_problem* p : g->problems) {
+      g->n_frames += p->n_frames;
+      g->n_points += p->n_points;
+    }
+    rc = group_attach(g, devs.data(), (int)devs.size());
+  }
+  if (rc != CLC_OK) {
+    const std::string msg = g_last_error;
+    clc_group_destroy(g);
+    g_last_error = msg;
+    return rc;
+  }
+  *out = g;
+  return CLC_OK;
+}
+
+// ---- trims: a new problem from the points of a device-resident one that lie near their board (clc_trim.cuh, clc_trim_plan.h) ----
+
+namespace {
+
+int check_trim(const double* pose7, int64_t n_frames, const double* max_abs_e) {
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(pose7[k])) return fail(CLC_ERR_INVALID, "pose7[" + std::to_string(k) + "] is not finite");
+  for (int64_t f = 0; f < n_frames; ++f)
+    if (!(max_abs_e[f] >= 0.0)) return fail(CLC_ERR_INVALID, "max_abs_e[" + std::to_string(f) + "] is NaN or negative");
+  return CLC_OK;
+}
+
+// The mark pass of one source shard.  One device buffer: kept points of every tile [n_tiles] and of every frame [n_frames] (next
+// to each other, so that one copy brings both to the host), the thresholds [n_frames], the keep mask [n_tiles * kTrimWords].
+struct TrimMarks {
+  int64_t* d_block = nullptr;
+  int64_t n_tiles = 0, n_frames = 0;
+  clc::TrimMarkArgs args = {};
+  std::vector<int64_t> counts;  // host copy: tile counts, then frame counts
+};
+
+int trim_mark_prepare(clc_problem* q, const double* pose7, const double* max_abs_e, TrimMarks* m) {
+  CLC_CUDA(cudaSetDevice(q->device));
+  m->n_tiles = (q->n_points + clc::kTrimTile - 1) / clc::kTrimTile;
+  m->n_frames = q->n_frames;
+  const int64_t words = 2 * m->n_frames + m->n_tiles + m->n_tiles * clc::kTrimWords / 2;
+  CLC_CUDA(cudaMallocAsync(&m->d_block, sizeof(int64_t) * std::max<int64_t>(words, 1), q->stream));
+  int64_t* frame_kept = m->d_block + m->n_tiles;
+  double* tau = reinterpret_cast<double*>(frame_kept + m->n_frames);
+  CLC_CUDA(cudaMemsetAsync(frame_kept, 0, sizeof(int64_t) * m->n_frames, q->stream));
+  if (m->n_frames > 0)
+    CLC_CUDA(cudaMemcpyAsync(tau, max_abs_e, sizeof(double) * m->n_frames, cudaMemcpyHostToDevice, q->stream));
+  clc::TrimMarkArgs& a = m->args;
+  a.x = q->x;
+  a.y = q->y;
+  a.z = q->z_all_zero ? nullptr : q->z;  // a z stream known to be all 0 (planar data on the general kernels) is not read
+  a.plane = q->plane;
+  a.offsets = q->offsets;
+  a.max_abs_e = tau;
+  a.n_frames = q->n_frames;
+  a.n_points = q->n_points;
+  for (int k = 0; k < 7; ++k) a.pose7[k] = pose7[k];
+  a.mask = reinterpret_cast<uint32_t*>(tau + m->n_frames);
+  a.tile_kept = m->d_block;
+  a.frame_kept = reinterpret_cast<unsigned long long*>(frame_kept);
+  // pageable host memory: the thresholds have been staged when the copy returns
+  return CLC_OK;
+}
+
+int trim_mark_launch(const TrimMarks& m, cudaStream_t stream) {
+  if (m.n_tiles == 0) return CLC_OK;
+  clc::clc_trim_mark_kernel<<<(unsigned)m.n_tiles, clc::kTrimThreads, 0, stream>>>(m.args);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the kept counts to the host (8 bytes per tile and frame)
+int trim_mark_collect(clc_problem* q, TrimMarks* m) {
+  CLC_CUDA(cudaSetDevice(q->device));
+  m->counts.resize((size_t)(m->n_tiles + m->n_frames));
+  if (!m->counts.empty())
+    CLC_CUDA(cudaMemcpyAsync(m->counts.data(), m->d_block, sizeof(int64_t) * m->counts.size(), cudaMemcpyDeviceToHost, q->stream));
+  CLC_CUDA(cudaStreamSynchronize(q->stream));
+  return CLC_OK;
+}
+
+void trim_marks_release(const std::vector<clc_problem*>& src, std::vector<TrimMarks>& marks) {
+  for (size_t s = 0; s < marks.size(); ++s)
+    if (marks[s].d_block && cudaSetDevice(src[s]->device) == cudaSuccess) cudaFreeAsync(marks[s].d_block, src[s]->stream);
+  marks.clear();
+}
+
+// Plans the trim from the kept counts and builds the shells of its destination shards, one per entry of `devices`, with the
+// gather's inputs uploaded (the source tiles' kept prefix and every destination tile's first source tile).
+int trim_prepare(const std::vector<clc_problem*>& src, const std::vector<TrimMarks>& marks, const std::vector<int>& devices,
+                 std::vector<SubsetShard>* out, std::vector<clc::TrimGatherArgs>* args) {
+  const int S = (int)src.size(), G = (int)devices.size();
+  std::vector<int64_t> src_frames((size_t)S), src_tiles((size_t)S);
+  std::vector<const int64_t*> frame_kept((size_t)S), tile_kept((size_t)S);
+  clc::TrimGatherArgs base = {};
+  base.n_src = S;
+  bool edges = false;
+  for (int s = 0; s < S; ++s) {
+    const clc_problem* q = src[s];
+    src_frames[s] = marks[s].n_frames;
+    src_tiles[s] = marks[s].n_tiles;
+    tile_kept[s] = marks[s].counts.data();
+    frame_kept[s] = marks[s].counts.data() + marks[s].n_tiles;
+    base.src[s] = {q->x, q->y, q->z_all_zero ? nullptr : q->z, marks[s].args.mask, q->frame_pose, q->edge_pt, q->frame_pose_true};
+    base.src_tile_begin[s + 1] = base.src_tile_begin[s] + src_tiles[s];
+    base.src_frame_begin[s + 1] = base.src_frame_begin[s] + src_frames[s];
+    edges = edges || q->n_edges > 0;
+  }
+  const clc::TrimPlan plan = clc::trim_plan(S, src_frames.data(), frame_kept.data(), src_tiles.data(), tile_kept.data(), G);
+  const bool true_poses = src[0]->frame_pose_true != nullptr;
+  out->assign((size_t)G, SubsetShard());
+  args->assign((size_t)G, base);
+  for (int d = 0; d < G; ++d) {
+    SubsetShard& sh = (*out)[d];
+    const int64_t fb = plan.shard_frame[d], fe = plan.shard_frame[d + 1], N = fe - fb;
+    const int64_t p0 = plan.offsets[fb], P = plan.offsets[fe] - p0;
+    std::vector<int64_t> offsets((size_t)N + 1);
+    for (int64_t f = 0; f <= N; ++f) offsets[f] = plan.offsets[fb + f] - p0;
+    // a z stream when some kept point of the shard comes from a source whose z is not known to be all 0
+    for (int s = 0; s < S; ++s) {
+      const int64_t k0 = plan.tile_prefix[base.src_tile_begin[s]], k1 = plan.tile_prefix[base.src_tile_begin[s + 1]];
+      sh.gathers_z = sh.gathers_z || (base.src[s].z != nullptr && std::max(k0, p0) < std::min(k1, p0 + P));
+    }
+    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]->use_loss,
+                          src[0]->cauchy_a);
+    if (rc != CLC_OK) return rc;
+    clc_problem* p = sh.p;
+    const int64_t t_begin = plan.tile_begin[d], n_tiles = plan.tile_begin[d + 1] - t_begin;
+    std::vector<int64_t> work(plan.tile_prefix);
+    work.insert(work.end(), plan.first_tile.begin() + t_begin, plan.first_tile.begin() + t_begin + n_tiles);
+    CLC_CUDA(cudaMallocAsync(&sh.d_work, sizeof(int64_t) * work.size(), p->stream));
+    CLC_CUDA(cudaMemcpyAsync(sh.d_work, work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
+    clc::TrimGatherArgs& a = (*args)[d];
+    a.tile_prefix = sh.d_work;
+    a.first_tile = sh.d_work + plan.tile_prefix.size();
+    a.point_begin = p0;
+    a.n_points = P;
+    a.n_tiles = n_tiles;
+    a.frame_begin = fb;
+    a.n_frames = N;
+    a.x = p->x;
+    a.y = p->y;
+    a.z = p->z;
+    a.frame_pose = p->frame_pose;
+    a.edge_pt = p->edge_pt;
+    a.frame_pose_true = p->frame_pose_true;
+    a.nonplanar = p->d_nonplanar;
+    // pageable host memory: the copies above have been staged when they return, the host vectors may go
+  }
+  return CLC_OK;
+}
+
+int trim_launch(const clc::TrimGatherArgs& a, cudaStream_t stream) {
+  const int64_t blocks = a.n_tiles + (a.n_frames + clc::kTrimThreads - 1) / clc::kTrimThreads;
+  if (blocks == 0) return CLC_OK;
+  clc::clc_trim_gather_kernel<<<(unsigned)blocks, clc::kTrimThreads, 0, stream>>>(a);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the whole trim: mark every source shard, plan, shells, one gather per destination shard (all devices in flight), finish
+int trim_build(const std::vector<clc_problem*>& src, const double* pose7, const double* max_abs_e, const std::vector<int>& devices,
+               std::vector<clc_problem*>* out) {
+  if (src.size() > (size_t)clc::kMaxRanks) return fail(CLC_ERR_INVALID, "too many source shards");
+  std::vector<TrimMarks> marks(src.size());
+  int rc = CLC_OK;
+  int64_t f0 = 0;
+  for (size_t s = 0; s < src.size() && rc == CLC_OK; ++s) {
+    rc = trim_mark_prepare(src[s], pose7, max_abs_e + f0, &marks[s]);
+    if (rc == CLC_OK) rc = trim_mark_launch(marks[s], src[s]->stream);
+    f0 += src[s]->n_frames;
+  }
+  for (size_t s = 0; s < src.size() && rc == CLC_OK; ++s) rc = trim_mark_collect(src[s], &marks[s]);
+  std::vector<SubsetShard> shards;
+  std::vector<clc::TrimGatherArgs> args;
+  if (rc == CLC_OK) rc = trim_prepare(src, marks, devices, &shards, &args);
+  if (rc == CLC_OK) rc = gather_shards(src, devices, shards, [&](size_t d) { return trim_launch(args[d], shards[d].p->stream); });
+  // the gathers read the keep masks: they are complete before the masks go
+  for (SubsetShard& sh : shards)
+    if (sh.p && sh.p->stream && cudaSetDevice(sh.p->device) == cudaSuccess) {
+      const cudaError_t e = cudaStreamSynchronize(sh.p->stream);
+      if (e != cudaSuccess && rc == CLC_OK) rc = fail(CLC_ERR_CUDA, std::string("trim gather: ") + cudaGetErrorString(e));
+    }
+  trim_marks_release(src, marks);
+  return finish_shards(shards, rc, out);
+}
+
+}  // namespace
+
+int clc_problem_trim(const clc_problem* src, const double pose7[7], const double* max_abs_e, clc_problem** out) {
+  if (!src || !pose7 || !max_abs_e || !out) return fail(CLC_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  int rc = check_trim(pose7, src->n_frames, max_abs_e);
+  if (rc != CLC_OK) return rc;
+  std::vector<clc_problem*> ps;
+  rc = trim_build({const_cast<clc_problem*>(src)}, pose7, max_abs_e, {src->device}, &ps);
+  if (rc != CLC_OK) return rc;
+  *out = ps[0];
+  return CLC_OK;
+}
+
+int clc_group_trim(const clc_group* src, const double pose7[7], const double* max_abs_e, clc_group** out) {
+  if (!src || !pose7 || !max_abs_e || !out) return fail(CLC_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  if (src->problems.empty()) return fail(CLC_ERR_INVALID, "empty group");
+  int rc = check_trim(pose7, src->n_frames, max_abs_e);
+  if (rc != CLC_OK) return rc;
+  std::vector<int> devs;
+  for (const clc_problem* p : src->problems) devs.push_back(p->device);
+  clc_group* g = new clc_group();
+  rc = trim_build(src->problems, pose7, max_abs_e, devs, &g->problems);
   if (rc == CLC_OK) {
     for (const clc_problem* p : g->problems) {
       g->n_frames += p->n_frames;
@@ -2624,6 +2853,37 @@ int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2,
     if (rc == CLC_OK) rc = set_device(p);
     if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &ms_each[i], [&]() { return subset_launch(shards[0], p->stream); });
     const std::string msg = g_last_error;
+    subset_release(shards);
+    g_last_error = msg;
+  }
+  return rc;
+}
+
+int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_abs_e, int n, int flush_l2, float* mark_ms,
+                   float* gather_ms) {
+  if (!src || !pose7 || !max_abs_e || n < 1 || !mark_ms || !gather_ms) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_trim(pose7, src->n_frames, max_abs_e);
+  if (rc != CLC_OK) return rc;
+  clc_problem* p = src;
+  rc = set_device(p);
+  int flush_smem = 0;
+  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
+  for (int i = 0; i < n && rc == CLC_OK; ++i) {
+    // a fresh mark and scratch problem every time; both passes run on the source's stream, each behind its own L2 flush
+    std::vector<TrimMarks> marks(1);
+    std::vector<SubsetShard> shards;
+    std::vector<clc::TrimGatherArgs> args;
+    rc = trim_mark_prepare(p, pose7, max_abs_e, &marks[0]);
+    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &mark_ms[i], [&]() { return trim_mark_launch(marks[0], p->stream); });
+    if (rc == CLC_OK) rc = trim_mark_collect(p, &marks[0]);
+    if (rc == CLC_OK) rc = trim_prepare({p}, marks, {p->device}, &shards, &args);
+    if (rc == CLC_OK) rc = shards[0].p->stream && cudaStreamSynchronize(shards[0].p->stream) == cudaSuccess
+                                ? CLC_OK : fail(CLC_ERR_CUDA, "scratch problem");
+    if (rc == CLC_OK) rc = set_device(p);
+    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &gather_ms[i], [&]() { return trim_launch(args[0], p->stream); });
+    const std::string msg = g_last_error;
+    if (set_device(p) == CLC_OK) cudaStreamSynchronize(p->stream);
+    trim_marks_release({p}, marks);
     subset_release(shards);
     g_last_error = msg;
   }

@@ -38,6 +38,12 @@ CLC_HD void frame_consts(const PoseConsts& pc, const double* plane, double* m, d
   *c = (n0 * pc.t[0] + n1 * pc.t[1] + n2 * pc.t[2]) + plane[3];
 }
 
+// The raw point-to-plane distance e = m.p + c of one point, rounded exactly as the sweep kernel and the frame report round it
+// (a point of a planar problem has z = 0: fma(m2, 0, c) == c).  The trim's thresholds compare against this value.
+CLC_HD double point_distance(const double* m, double c, double x, double y, double z) {
+  return fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
+}
+
 // Moments layout: S[0]=S0, S[1..3]=S1 (x,y,z), S[4..9]=S2 (xx,xy,xz,yy,yz,zz).
 // Adds the piece's contribution to out[28] = 21 upper-tri H (row-major, i<=j), 6 g, 1 cost.
 //   s2        = 1/(#points of the whole frame)

@@ -313,6 +313,28 @@ int clc_problem_subset(const clc_problem* src, const uint8_t* keep, clc_problem*
  * each source device's default memory pool is opened to the other devices of the group (cudaMemPoolSetAccess) and closed again
  * afterwards, unless the caller had already granted that access. */
 int clc_group_subset(const clc_group* src, const uint8_t* keep, clc_group** out);
+/* ---- trims: solve again without the points that lie far from their board, without sending the points through the host again --
+ * A new problem on src's device holding, of every frame f of src, the points whose raw point-to-plane distance at pose7 satisfies
+ * |e| <= max_abs_e[f] (max_abs_e has src's n_frames entries).  e is computed exactly as the sweep kernel and clc_frame_report
+ * compute it -- m = R^T n, c = n.t + d from pose7 and the frame's board plane, e = fma(m0, x, fma(m1, y, fma(m2, z, c))) -- so
+ * the report's max_abs_e and the threshold are the same quantity.  A NaN e is never kept; max_abs_e[f] = +inf keeps every point of
+ * frame f whose e is not NaN.  Every frame is kept, in order, with its pose, its edge points (the front and back points of the raw
+ * scan, which are not trimmed) and (synthetic camera-mode sources) its true pose; a frame may end up empty (clc_problem_subset
+ * removes such frames).  Only the kept counts of every frame and of every 2048-point tile come to the host; a mark kernel and a
+ * gather kernel do the rest.  The result is the problem clc_problem_create would build from src's frame poses, the kept points and
+ * src's edge points -- the same layout, planes, planarity verdict, kernel family, partition and dispatch, so every output is
+ * bit-identical to that fresh problem's.  In particular the per-frame scale s = 1/sqrt(#points of the frame) follows the new point
+ * counts (reference src/LaseCamCalCeres.cpp:239-240), and a problem whose only z != 0 were trimmed is planar when it is large
+ * enough.  The +-0.0 exception of clc_problem_subset applies unchanged.  It inherits use_loss and cauchy_a; it starts in the
+ * default planar mode and is attached to no communicator.  src is unchanged and stays valid; both need device memory at once.
+ * A NULL argument, a pose7 entry that is not finite or a max_abs_e entry that is NaN or negative fails with CLC_ERR_INVALID
+ * before the device is touched. */
+int clc_problem_trim(const clc_problem* src, const double pose7[7], const double* max_abs_e, clc_problem** out);
+/* The same for an in-process group (max_abs_e: one entry per frame of the group, in the global frame order): a new group on the
+ * same device list, the trimmed frames re-sharded over it by their new point counts as clc_group_create_gather shards a fresh
+ * problem, so shard boundaries move and kept points may cross devices.  They are read over the peer links under the same
+ * temporary memory-pool grants as clc_group_subset's. */
+int clc_group_trim(const clc_group* src, const double pose7[7], const double* max_abs_e, clc_group** out);
 /* The device list the reference-facing drop-in uses (its signatures have no device argument): environment variable
  * CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device only).  Writes at most `cap` ordinals. */
 int clc_default_devices(int* devices, int cap, int* n);
@@ -329,6 +351,12 @@ int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flu
  * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
  * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
 int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2, float* ms_each);
+/* The two device passes of clc_problem_trim(src, pose7, max_abs_e): `n` times the mark kernel is timed (CUDA events, after the L2
+ * flush when flush_l2 != 0), the kept counts come to the host and a scratch trim is prepared, then its gather kernel is timed the
+ * same way and the scratch problem is destroyed.  mark_ms[n] and gather_ms[n] receive the device times; the host step between
+ * the passes is in neither.  Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
+int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_abs_e, int n, int flush_l2, float* mark_ms,
+                   float* gather_ms);
 /* Algorithmic bytes of one K1 launch on this problem: 24*P + 40*N + 56*edges + 224 (SURVEY.md section 8(d)). */
 int clc_problem_algorithmic_bytes(const clc_problem* p, int64_t* bytes);
 /* Bytes one K1 launch actually streams: the figure above with 16 instead of 24 bytes per point when the planar
