@@ -183,6 +183,24 @@ def _thresholds(max_abs_e, n_frames):
     return np.ascontiguousarray(t)
 
 
+def _segments(seg_offsets, poses, n_frames):
+    """A segmentation seg_offsets [W + 1] of n_frames frames and one pose7 per segment [W, 7] -> the int64 / float64 arrays of the
+    C ABI (checked before any device work: the library checks them too)."""
+    off = np.asarray(seg_offsets)
+    if off.ndim != 1 or off.size < 2 or not np.issubdtype(off.dtype, np.integer):
+        raise ValueError("seg_offsets must be a 1-D integer array of at least 2 entries")
+    off = np.ascontiguousarray(off, dtype=np.int64)
+    if off[0] != 0 or off[-1] != n_frames or np.any(np.diff(off) < 0):
+        raise ValueError(f"seg_offsets must start at 0, not decrease and end at n_frames = {n_frames}")
+    W = off.size - 1
+    x = np.ascontiguousarray(poses, dtype=np.float64)
+    if x.shape != (W, 7):
+        raise ValueError(f"poses must have shape ({W}, 7), not {x.shape}")
+    if not np.all(np.isfinite(x)):
+        raise ValueError("poses must be finite")
+    return off, x, W
+
+
 def default_options(**kw) -> LmOptions:
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
@@ -383,6 +401,41 @@ class Problem:
         information()'s chi."""
         return _frame_report(self._L.clc_frame_report, self._h, self.sizes()[0], pose7, "clc_frame_report")
 
+    # ---- independent solves over runs of frames (segments) ----
+    def eval_segments(self, seg_offsets, poses):
+        """eval() of every segment [seg_offsets[s], seg_offsets[s + 1]) of the frames at its own pose poses[s], from ONE shared
+        sweep (clc_eval_segments).  Returns (cost [W], H [W, 6, 6], g [W, 6]); segment s's are those of a fresh problem of its
+        frames alone, up to the order of summation."""
+        off, x, W = _segments(seg_offsets, poses, self.sizes()[0])
+        cost, H, g = np.empty(W), np.empty((W, 6, 6)), np.empty((W, 6))
+        _lib.check(self._L.clc_eval_segments(self._h, W, _ip(off), _dp(x), _dp(H), _dp(g), _dp(cost)), "clc_eval_segments")
+        return cost, H, g
+
+    def information_segments(self, seg_offsets, poses):
+        """information() of every segment at its own pose (clc_information_segments): (H [W, 6, 6], b [W, 6], chi [W], sv [W, 6]);
+        the right singular vectors go to self.last_V [W, 6, 6]."""
+        off, x, W = _segments(seg_offsets, poses, self.sizes()[0])
+        H, b, chi, sv = np.empty((W, 6, 6)), np.empty((W, 6)), np.empty(W), np.empty((W, 6))
+        self.last_V = np.empty((W, 6, 6))
+        _lib.check(self._L.clc_information_segments(self._h, W, _ip(off), _dp(x), _dp(H), _dp(b), _dp(chi), _dp(sv),
+                                                    _dp(self.last_V)), "clc_information_segments")
+        return H, b, chi, sv
+
+    def solve_segments(self, seg_offsets, poses, options: LmOptions | None = None, trace_cap=0):
+        """solve() of every segment from its own start pose poses[s], W solves advancing side by side on shared sweeps
+        (clc_solve_lm_segments).  Returns (poses [W, 7], summaries [W] of LmSummary, traces: one list of LmIteration per segment,
+        empty without trace_cap).  summaries[s].device_ms is the time of the whole segmented solve."""
+        off, x, W = _segments(seg_offsets, poses, self.sizes()[0])
+        x = x.copy()
+        o = options if options is not None else default_options()
+        summaries = (LmSummary * W)()
+        tr = (LmIteration * (W * trace_cap))() if trace_cap > 0 else None
+        _lib.check(self._L.clc_solve_lm_segments(self._h, W, _ip(off), _dp(x), C.byref(o), summaries, tr, int(trace_cap)),
+                   "clc_solve_lm_segments")
+        traces = [[tr[s * trace_cap + i] for i in range(min(summaries[s].num_iterations, trace_cap))] if trace_cap > 0 else []
+                  for s in range(W)]
+        return x, list(summaries), traces
+
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()
         _lib.check(self._L.clc_closed_form(self._h, _dp(T), C.byref(un), _dp(AtA), _dp(Atb)), "clc_closed_form")
@@ -418,6 +471,14 @@ class Problem:
         pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_frame_report(self._h, _dp(pose7), int(n), int(bool(flush_l2)), ms), "clc_bench_frame_report")
+        return np.array(ms[:], dtype=np.float64)
+
+    def bench_segments(self, seg_offsets, poses, n, flush_l2=True):
+        """Device time of n iterations of the segmented calls (frame constants, segment sweep, fix-up, two-level reduction;
+        clc_bench_segments), ms each."""
+        off, x, W = _segments(seg_offsets, poses, self.sizes()[0])
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_segments(self._h, W, _ip(off), _dp(x), int(n), int(bool(flush_l2)), ms), "clc_bench_segments")
         return np.array(ms[:], dtype=np.float64)
 
     def bench_subset(self, keep, n, flush_l2=True):

@@ -24,6 +24,7 @@
 #include "clc_kernels.cuh"
 #include "clc_l2_plan.h"
 #include "clc_linefit.cuh"
+#include "clc_segments.cuh"
 #include "clc_small.cuh"
 #include "clc_subset.cuh"
 #include "clc_subset_plan.h"
@@ -326,7 +327,7 @@ int set_device(const clc_problem* p) {
 // kModeFrames: frame_rows / frame_slots receive the per-frame report (clc_frame_fixup_kernel finishes it)
 int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* d_pose, const int* d_done,
                  clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false,
-                 double* frame_rows = nullptr, double* frame_slots = nullptr) {
+                 double* frame_rows = nullptr, double* frame_slots = nullptr, const double* seg_consts = nullptr) {
   clc::SweepArgs a;
   a.pose7 = d_pose;
   a.done = d_done;
@@ -346,6 +347,7 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   a.error = p->p2p_error;
   a.frame_rows = frame_rows;
   a.frame_slots = frame_slots;
+  a.seg_consts = seg_consts;
   if (p->nranks > 1 && p->allreduce_mode == 1 && collective) {
     clc_comm* c = p->comm_obj;
     a.nranks = c->nranks;
@@ -374,6 +376,16 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
     void (*fn)(clc::ProblemView, clc::SweepArgs) =
         loss ? (p->planar ? clc::clc_sweep_kernel<true, clc::kModeFrames, true> : clc::clc_sweep_kernel<true, clc::kModeFrames, false>)
              : (p->planar ? clc::clc_sweep_kernel<false, clc::kModeFrames, true> : clc::clc_sweep_kernel<false, clc::kModeFrames, false>);
+    CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+    le = cudaLaunchKernelEx(&cfg, fn, v, a);
+  } else if (mode == clc::kModeSegments) {
+    // the segmented solves: no LM state in the kernel, no L2 hints, never collective
+    if (frame_rows == nullptr || frame_slots == nullptr || seg_consts == nullptr || d_lm != nullptr || loop_sweeps > 1 ||
+        a.nranks > 1)
+      return fail(CLC_ERR_INVALID, "internal: bad segmented sweep");
+    void (*fn)(clc::ProblemView, clc::SweepArgs) =
+        loss ? (p->planar ? clc::clc_sweep_kernel<true, clc::kModeSegments, true> : clc::clc_sweep_kernel<true, clc::kModeSegments, false>)
+             : (p->planar ? clc::clc_sweep_kernel<false, clc::kModeSegments, true> : clc::clc_sweep_kernel<false, clc::kModeSegments, false>);
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
   } else if (mode == clc::kModeClosedForm) {
@@ -1524,6 +1536,230 @@ int clc_solve_lm(clc_problem* p, double pose7[7], const clc_lm_options* opt_in, 
                  clc_lm_iteration* trace, int trace_cap) {
   if (!p || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
   return solve_all(&p, 1, pose7, opt_in, summary, trace, trace_cap);
+}
+
+// ---- independent solves over runs of frames (segments) ----------------------------------------------------------------
+// Every problem size runs them on the sweep kernel K1 (kModeSegments) with the kernel family eval uses; clc_segments.cuh has the
+// kernels of one iteration and clc_segment_plan.h the segmentation and its reduction plan.
+
+namespace {
+
+// rejects bad arguments before the device is touched
+int check_segments(const clc_problem* p, int64_t W, const int64_t* seg_offsets, const double* poses) {
+  if (!p || !seg_offsets || !poses) return fail(CLC_ERR_INVALID, "NULL argument");
+  if (W < 1) return fail(CLC_ERR_INVALID, "n_segments < 1");
+  if (!clc::segments_valid(p->n_frames, W, seg_offsets))
+    return fail(CLC_ERR_INVALID, "seg_offsets must start at 0, not decrease and end at n_frames");
+  for (int64_t i = 0; i < 7 * W; ++i)
+    if (!clc::is_finite(poses[i])) return fail(CLC_ERR_INVALID, "a pose entry is not finite");
+  if (p->comm_obj != nullptr || p->nranks > 1) return fail(CLC_ERR_STATE, "segmented solves run on a problem without a communicator");
+  return CLC_OK;
+}
+
+// The device buffers of one segmented call (freed on the problem's stream when it ends).
+struct SegmentRun {
+  clc_problem* p = nullptr;
+  int64_t W = 0, n_chunks = 0;
+  int32_t* frame_seg = nullptr;
+  int64_t* chunk_offsets = nullptr;
+  int64_t* seg_chunks = nullptr;
+  double* consts = nullptr;    // [(n_frames + n_edges) * 4]
+  double* raw = nullptr;       // [n_frames * kSegRawDoubles] the sweep's raw row of every whole frame
+  double* rows = nullptr;      // [n_frames * kNumSums]
+  double* slots = nullptr;     // [grid * kWarps * 2 * kSlotDoubles]
+  double* partials = nullptr;  // [n_chunks * kNumSums]
+  double* poses = nullptr;     // [W * 7] eval / information
+  double* sums = nullptr;      // [W * kNumSums] eval / information
+  clc::LmCore* cores = nullptr;    // [W] solve
+  clc_lm_iteration* trace = nullptr;  // [W * trace_cap] solve with a trace
+  int* counters = nullptr;     // [2] solve: segments still running, all done
+  ~SegmentRun() {
+    if (!p) return;
+    cudaSetDevice(p->device);
+    for (void* b : {(void*)frame_seg, (void*)chunk_offsets, (void*)seg_chunks, (void*)consts, (void*)raw, (void*)rows, (void*)slots,
+                    (void*)partials, (void*)poses, (void*)sums, (void*)cores, (void*)trace, (void*)counters})
+      if (b) cudaFreeAsync(b, p->stream);
+  }
+};
+
+int seg_alloc_bytes(clc_problem* p, void** out, size_t bytes) {
+  CLC_CUDA(cudaMallocAsync(out, std::max<size_t>(bytes, 8), p->stream));
+  return CLC_OK;
+}
+#define seg_alloc(p, out, n) seg_alloc_bytes((p), reinterpret_cast<void**>(out), sizeof(**(out)) * (size_t)(n))
+
+// the plan, the work buffers and the problem's eval pose (which the sweep does not use) on the device
+int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, SegmentRun* r) {
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  r->p = p;
+  r->W = W;
+  const clc::SegmentPlan plan = clc::segment_plan(p->n_frames, W, seg_offsets);
+  r->n_chunks = (int64_t)plan.chunk_offsets.size() - 1;
+  const size_t N = (size_t)p->n_frames;
+  if ((rc = seg_alloc(p, &r->frame_seg, N)) != CLC_OK || (rc = seg_alloc(p, &r->chunk_offsets, plan.chunk_offsets.size())) != CLC_OK ||
+      (rc = seg_alloc(p, &r->seg_chunks, plan.seg_chunks.size())) != CLC_OK ||
+      (rc = seg_alloc(p, &r->consts, (N + (size_t)p->n_edges) * 4)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->raw, N * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->rows, N * clc::kNumSums)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->slots, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->partials, (size_t)r->n_chunks * clc::kNumSums)) != CLC_OK)
+    return rc;
+  // pageable sources: each copy has read its source when it returns
+  if (N > 0) CLC_CUDA(cudaMemcpyAsync(r->frame_seg, plan.frame_seg.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->chunk_offsets, plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
+                           cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->seg_chunks, plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(), cudaMemcpyHostToDevice,
+                           p->stream));
+  return CLC_OK;
+}
+
+// One shared sweep of every segment: pose s at poses[s * pose_stride] on the device.  sums: [W * kNumSums] or nullptr; cores:
+// the solve's LmCores (lm_update runs on every segment that has not terminated), with its trace, counters and `done` flag.
+int segments_iteration(const SegmentRun& r, bool loss, bool edges, const double* poses, int64_t pose_stride, double* sums,
+                       clc::LmCore* cores, clc_lm_iteration* trace, int trace_cap, int* counters) {
+  clc_problem* p = r.p;
+  int* done = counters != nullptr ? counters + 1 : nullptr;  // raised when every segment has terminated
+  const bool with_edges = edges && p->n_edges > 0;
+  const clc::ProblemView v = make_view(p);
+  const int threads = 256;
+  if (p->n_frames > 0) {
+    const unsigned fb = (unsigned)((p->n_frames + threads - 1) / threads);
+    clc::clc_segment_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.frame_seg, poses, pose_stride, with_edges ? 1 : 0, done,
+                                                                  r.consts);
+    CLC_LAUNCH_CHECK();
+    int rc = launch_sweep(p, clc::kModeSegments, loss, with_edges, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
+                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.raw, r.slots, r.consts);
+    if (rc != CLC_OK) return rc;
+    if (loss)
+      clc::clc_segment_fixup_kernel<true><<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
+    else
+      clc::clc_segment_fixup_kernel<false><<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
+    CLC_LAUNCH_CHECK();
+  }
+  if (r.n_chunks > 0) {
+    const unsigned cb = (unsigned)((r.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+    clc::clc_segment_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.rows, r.chunk_offsets, r.n_chunks, done,
+                                                                                     r.partials);
+    CLC_LAUNCH_CHECK();
+  }
+  const unsigned sb = (unsigned)((r.W + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+  clc::clc_segment_lm_kernel<<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.partials, r.seg_chunks, r.W, sums, cores, trace,
+                                                                                trace_cap, counters, done);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the per-segment sums of one shared sweep at the poses [W * 7] (which: 0 eval, 1 information -- no loss, no edges)
+int eval_segments_run(clc_problem* p, int64_t W, const int64_t* seg_offsets, const double* poses, int which,
+                      std::vector<double>* sums) {
+  int rc = check_segments(p, W, seg_offsets, poses);
+  if (rc != CLC_OK) return rc;
+  SegmentRun r;
+  if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK) return rc;
+  if ((rc = seg_alloc(p, &r.poses, (size_t)W * 7)) != CLC_OK || (rc = seg_alloc(p, &r.sums, (size_t)W * clc::kNumSums)) != CLC_OK)
+    return rc;
+  CLC_CUDA(cudaMemcpyAsync(r.poses, poses, sizeof(double) * 7 * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  const bool loss = which == 0 && p->use_loss != 0, edges = which == 0 && p->n_edges > 0;
+  rc = segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
+  if (rc != CLC_OK) return rc;
+  sums->resize((size_t)W * clc::kNumSums);
+  CLC_CUDA(cudaMemcpyAsync(sums->data(), r.sums, sizeof(double) * sums->size(), cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  return CLC_OK;
+}
+
+}  // namespace
+
+int clc_eval_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36, double* g6,
+                      double* cost) {
+  if (!cost) return fail(CLC_ERR_INVALID, "NULL argument");
+  std::vector<double> sums;
+  int rc = eval_segments_run(p, n_segments, seg_offsets, poses, 0, &sums);
+  if (rc != CLC_OK) return rc;
+  for (int64_t s = 0; s < n_segments; ++s)
+    eval_post(sums.data() + s * clc::kNumSums, H36 ? H36 + 36 * s : nullptr, g6 ? g6 + 6 * s : nullptr, cost + s);
+  return CLC_OK;
+}
+
+int clc_information_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36,
+                             double* b6, double* chi, double* singular_values6, double* V36) {
+  std::vector<double> sums;
+  int rc = eval_segments_run(p, n_segments, seg_offsets, poses, 1, &sums);
+  if (rc != CLC_OK) return rc;
+  for (int64_t s = 0; s < n_segments; ++s)
+    information_post(sums.data() + s * clc::kNumSums, H36 ? H36 + 36 * s : nullptr, b6 ? b6 + 6 * s : nullptr, chi ? chi + s : nullptr,
+                     singular_values6 ? singular_values6 + 6 * s : nullptr, V36 ? V36 + 36 * s : nullptr);
+  return CLC_OK;
+}
+
+int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, double* poses, const clc_lm_options* opt_in,
+                          clc_lm_summary* summaries, clc_lm_iteration* trace, int trace_cap) {
+  if (!summaries || trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
+    return fail(CLC_ERR_INVALID, "NULL summaries, or trace_cap outside [0, 256] without a trace array");
+  int rc = check_segments(p, n_segments, seg_offsets, poses);
+  if (rc != CLC_OK) return rc;
+  clc_lm_options opt;
+  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
+  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
+  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  const int64_t W = n_segments;
+  SegmentRun r;
+  if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK || (rc = seg_alloc(p, &r.cores, (size_t)W)) != CLC_OK ||
+      (rc = seg_alloc(p, &r.counters, 2)) != CLC_OK)
+    return rc;
+  if (trace_cap > 0 && (rc = seg_alloc(p, &r.trace, (size_t)W * trace_cap)) != CLC_OK) return rc;
+  std::vector<clc::LmCore> cores((size_t)W);
+  for (int64_t s = 0; s < W; ++s) clc::lm_init(&cores[s], poses + 7 * s, opt);
+  CLC_CUDA(cudaMemcpyAsync(r.cores, cores.data(), sizeof(clc::LmCore) * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  const int counters0[2] = {(int)W, 0};
+  CLC_CUDA(cudaMemcpyAsync(r.counters, counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  // the candidate pose of segment s: cores[s].cand, sizeof(LmCore) / 8 doubles apart
+  const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.cores) + offsetof(clc::LmCore, cand));
+  const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
+  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
+  const int max_sweeps = opt.max_num_iterations + 2;
+  int launched = 0;
+  while (launched < max_sweeps) {
+    // the first batch is twice as long, as in solve_all
+    const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
+    for (int i = 0; i < batch; ++i) {
+      rc = segments_iteration(r, loss, edges, cand, stride, nullptr, r.cores, r.trace, trace_cap, r.counters);
+      if (rc != CLC_OK) return rc;
+    }
+    launched += batch;
+    CLC_CUDA(cudaMemcpyAsync(p->h_done, r.counters, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(sync_stream_low_latency(p->stream));
+    if (*p->h_done == 0) break;  // no segment is running
+  }
+  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(cores.data(), r.cores, sizeof(clc::LmCore) * (size_t)W, cudaMemcpyDeviceToHost, p->stream));
+  std::vector<clc_lm_iteration> rows((size_t)W * trace_cap);
+  if (trace_cap > 0)
+    CLC_CUDA(cudaMemcpyAsync(rows.data(), r.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  float ms = 0.f;
+  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
+  for (int64_t s = 0; s < W; ++s) {
+    const clc::LmCore& c = cores[s];
+    for (int i = 0; i < 7; ++i) poses[7 * s + i] = c.x[i];  // the last accepted point, as clc_solve_lm
+    clc_lm_summary& sm = summaries[s];
+    sm.termination = c.done ? c.done : CLC_TERM_NO_CONVERGENCE;
+    sm.num_iterations = c.n_trace;
+    sm.num_successful_steps = c.num_successful;
+    sm.num_unsuccessful_steps = c.num_unsuccessful;
+    sm.num_sweeps = c.sweeps;
+    sm.reserved = 0;
+    sm.initial_cost = c.initial_cost;
+    sm.final_cost = c.x_cost;
+    sm.device_ms = ms;
+    const int n = std::min(c.n_trace, trace_cap);
+    for (int i = 0; i < n; ++i) trace[s * trace_cap + i] = rows[(size_t)s * trace_cap + i];
+  }
+  return CLC_OK;
 }
 
 // ---- LineFittingCeres, batched ------------------------------------------------------------------------------------
@@ -2817,6 +3053,26 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
   const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
   return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
     return launch_sweep(p, clc::kModeLM, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false);
+  });
+}
+
+int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, int n, int flush_l2,
+                       float* ms_each) {
+  if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_segments(p, n_segments, seg_offsets, poses);
+  if (rc != CLC_OK) return rc;
+  SegmentRun r;
+  if ((rc = segments_prepare(p, n_segments, seg_offsets, &r)) != CLC_OK ||
+      (rc = seg_alloc(p, &r.poses, (size_t)n_segments * 7)) != CLC_OK ||
+      (rc = seg_alloc(p, &r.sums, (size_t)n_segments * clc::kNumSums)) != CLC_OK)
+    return rc;
+  CLC_CUDA(cudaMemcpyAsync(r.poses, poses, sizeof(double) * 7 * (size_t)n_segments, cudaMemcpyHostToDevice, p->stream));
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
+  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
+    return segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
   });
 }
 

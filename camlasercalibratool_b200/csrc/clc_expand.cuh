@@ -132,10 +132,9 @@ CLC_HD void accumulate_residual(const PoseConsts& pc, const double* plane, doubl
 
 // One board-edge residual (plane = an edge plane, pt = its edge point) expanded through its moments into out[28], as the edge
 // tail of the sweep kernel does; returns the raw distance e.  s2 = 1/#points of the frame.
-CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const double* pt, double s2, bool use_loss, double a2,
-                            double inv_a2, double* out) {
-  double m[3], c;
-  frame_consts(pc, plane, m, &c);
+// m, c: the edge plane's constants at the pose (frame_consts).
+CLC_HD double edge_residual_at(const double* plane, const double* m, double c, const double* pt, double s2, bool use_loss,
+                               double a2, double inv_a2, double* out) {
   const double x = pt[0], y = pt[1], z = pt[2];
   const double e = fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
   double w = 1.0, cost_term = e * e;
@@ -147,6 +146,14 @@ CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const dou
   const double S[10] = {w, w * x, w * y, w * z, w * x * x, w * x * y, w * x * z, w * y * y, w * y * z, w * z * z};
   expand_lm(plane, m, c, s2, S, use_loss, cost_term, a2, out);
   return e;
+}
+
+// edge_residual_at with m, c = frame_consts(pc, plane)
+CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const double* pt, double s2, bool use_loss, double a2,
+                            double inv_a2, double* out) {
+  double m[3], c;
+  frame_consts(pc, plane, m, &c);
+  return edge_residual_at(plane, m, c, pt, s2, use_loss, a2, inv_a2, out);
 }
 
 // Closed-form initialisation (reference src/LaseCamCalCeres.cpp:144-161): row A_k = n (x) (x, y, 1), b_k = -d, so

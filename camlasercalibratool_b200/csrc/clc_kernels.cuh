@@ -77,7 +77,12 @@ __host__ __device__ constexpr int frames_smem_bytes(bool planar) {
 
 // kModeFrames: the per-frame report (clc_frame_report) -- every frame's residual statistics and its share of the normal
 // equations go to a row of their own instead of being summed
-enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2 };
+// kModeSegments: independent solves over runs of frames (clc_*_segments) -- every frame's raw moments at its segment's pose go
+// to a row of their own (clc_segment_fixup_kernel expands them); the frame constants m, c come from SweepArgs::seg_consts.
+// A raw row: 10 moments, the cost (loss: product of (1 + e^2/a^2) with its exponent taken out; no loss: sum e^2) and that
+// exponent -- the layout of the first 12 doubles of a split-frame slot.
+constexpr int kSegRawDoubles = 12;
+enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3 };
 
 // Device-resident problem (read-only for the sweeps).
 struct ProblemView {
@@ -128,6 +133,8 @@ struct SweepArgs {
   // kModeFrames only
   double* frame_rows;   // [n_frames * kRowDoubles] the report rows of the frames that lie in one warp range
   double* frame_slots;  // [total warps * 2 * kSlotDoubles] head / tail pieces of split frames (clc_frames.cuh)
+  // kModeSegments only (frame_rows then holds [n_frames * kSegRawDoubles] raw rows; frame_slots as above)
+  const double* seg_consts;  // [(n_frames + n_edges) * 4] m, c of every frame, then of every edge residual, at its segment's pose
 };
 
 // ---- small device helpers ---------------------------------------------------------------------------------
@@ -248,6 +255,27 @@ __device__ __forceinline__ void warp_transpose_sum(double* v, int lane) {
       v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
     }
   }
+#pragma unroll
+  for (int o = N; o < 32; o <<= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
+}
+
+// warp_transpose_sum with every round a template instance: the trip counts are compile-time constants, so the rounds unroll
+// completely and v stays in registers (warp_transpose_sum's loop over a shifted bound is not fully unrolled, which sends v to
+// local memory).  kModeSegments uses it so that nothing goes through local memory in the streaming loop.
+template <int HALF>
+__device__ __forceinline__ void transpose_round(double* v, int lane) {
+  const bool upper = (lane & HALF) != 0;
+#pragma unroll
+  for (int i = 0; i < HALF; ++i) {
+    const double keep = upper ? v[i + HALF] : v[i];
+    const double send = upper ? v[i] : v[i + HALF];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
+  }
+  if constexpr (HALF > 1) transpose_round<HALF / 2>(v, lane);
+}
+template <int N>
+__device__ __forceinline__ void warp_transpose_sum_regs(double* v, int lane) {
+  transpose_round<N / 2>(v, lane);
 #pragma unroll
   for (int o = N; o < 32; o <<= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
 }
@@ -586,24 +614,31 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     double m0 = 0.0, m1 = 0.0, m2 = 0.0, c = 0.0;
     // frame constants (every lane, redundantly); the next frame's plane and end offset are prefetched one piece
     // ahead so that a frame change does not stall the stream on a global-memory round trip
+    // kModeSegments: every frame's m, c were computed at its segment's pose before the sweep; they take the place of its plane
+    const double* fsrc = pv.plane;
+    if constexpr (MODE == kModeSegments) fsrc = args.seg_consts;
     double nx_plane[4] = {0.0, 0.0, 0.0, 0.0};
     int64_t nx_end = 0;
     auto prefetch_next = [&]() {
       if (f + 1 < pv.n_frames) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k) nx_plane[k] = pv.plane[(f + 1) * 4 + k];
+        for (int k = 0; k < 4; ++k) nx_plane[k] = fsrc[(f + 1) * 4 + k];
         nx_end = pv.offsets[f + 2];
       }
     };
     auto set_frame_consts = [&](const double* plane) {
-      double m[3];
-      frame_consts(pc, plane, m, &c);
-      m0 = m[0]; m1 = m[1]; m2 = m[2];
+      if constexpr (MODE == kModeSegments) {
+        m0 = plane[0]; m1 = plane[1]; m2 = plane[2]; c = plane[3];
+      } else {
+        double m[3];
+        frame_consts(pc, plane, m, &c);
+        m0 = m[0]; m1 = m[1]; m2 = m[2];
+      }
     };
     {
       double plane[4];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) plane[k] = pv.plane[f * 4 + k];
+      for (int k = 0; k < 4; ++k) plane[k] = fsrc[f * 4 + k];
       set_frame_consts(plane);
       prefetch_next();
     }
@@ -635,6 +670,23 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         }
       } else {
         v[10] = pr;  // sum of e^2
+      }
+      if constexpr (MODE == kModeSegments) {
+        // every piece leaves raw -- the moments and the cost (loss: product and exponent): a whole frame to its row of
+        // kSegRawDoubles, a piece of a split frame to this warp's head or tail slot.  clc_segment_fixup_kernel expands them all,
+        // so no expansion state is live in the streaming loop, and the transpose keeps v in registers: nothing goes through
+        // local memory between the stage loop's head and its back-edges.
+        warp_transpose_sum_regs<16>(v, lane);
+        const int kind = frame_piece_kind(pv.offsets[f], f_end, p0, p1);
+        double* dst = kind == kPieceWhole
+                          ? args.frame_rows + f * kSegRawDoubles
+                          : args.frame_slots + (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kSlotDoubles;
+        if (lane < 10 || (!LOSS && lane == 10)) dst[lane] = v[0];
+        if (LOSS && lane == 10) dst[10] = pr;
+        if (lane == 11) dst[11] = (double)es;
+        moments_clear<LOSS>(a);
+        open = false;
+        return;
       }
       warp_transpose_sum<16>(v, lane);  // lane L: total of moment (L mod 16)
       const int kind = MODE == kModeFrames ? frame_piece_kind(pv.offsets[f], f_end, p0, p1) : (int)kPieceWhole;
@@ -704,7 +756,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
             if (f_end > q) {
               double plane[4];
 #pragma unroll
-              for (int k = 0; k < 4; ++k) plane[k] = pv.plane[f * 4 + k];
+              for (int k = 0; k < 4; ++k) plane[k] = fsrc[f * 4 + k];
               set_frame_consts(plane);
             }
           }
@@ -716,13 +768,24 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
           // the whole stage belongs to one frame: no masks
 #pragma unroll
           for (int g = 0; g < G; ++g) {
-            process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2);
+            process2<LOSS, MODE == kModeLM || MODE == kModeSegments, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2);
             if (MODE == kModeFrames) frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], true, true, m0, m1, m2, c);
           }
         } else {
 #pragma unroll
           for (int g = 0; g < G; ++g) {
             const int64_t i0 = cb + 64 * g + 2 * lane;
+            if constexpr (MODE == kModeSegments) {
+              // the points outside the piece may belong to another segment: their coordinates are replaced before any
+              // arithmetic (a NaN there must not reach this frame through 0 * NaN), so every segment's rows depend on its
+              // own points only
+              const bool v0 = i0 >= q && i0 < hi, v1 = i0 + 1 >= q && i0 + 1 < hi;
+              const double2 Xm = make_double2(v0 ? X[g].x : 0.0, v1 ? X[g].y : 0.0);
+              const double2 Ym = make_double2(v0 ? Y[g].x : 0.0, v1 ? Y[g].y : 0.0);
+              const double2 Zm = make_double2(v0 ? Z[g].x : 0.0, v1 ? Z[g].y : 0.0);
+              process2<LOSS, true, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, pv.inv_a2);
+              continue;
+            }
             process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2,
                                             c, pv.inv_a2);
             if (MODE == kModeFrames)
@@ -748,6 +811,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     flush_frames();
     return;
   }
+  if constexpr (MODE == kModeSegments) return;  // every piece has left raw (park_piece): no tile, no block reduction
   CLC_STAMP(1);
   if (args.timing != nullptr && lane == 0) args.timing[(int64_t)gridDim.x * 8 + gwarp] = globaltimer_ns();
   flush_tile();

@@ -84,6 +84,18 @@ CLC_HD void lm_record(LmCore* s, clc_lm_iteration* trace, const clc_lm_iteration
   s->n_trace++;
 }
 
+// A trace of `cap` rows (cap 0: none, rows may be NULL): the segmented solve (clc_solve_lm_segments) keeps one per segment and
+// allocates them only when the caller asks for a trace.
+struct TraceRows {
+  clc_lm_iteration* rows;
+  int cap;
+};
+
+CLC_HD void lm_record(LmCore* s, TraceRows trace, const clc_lm_iteration& it) {
+  if (s->n_trace < trace.cap) trace.rows[s->n_trace] = it;
+  s->n_trace++;
+}
+
 CLC_HD void lm_init(LmCore* s, const double* pose7, const clc_lm_options& opt) {
   s->done = 0; s->phase = 0; s->iteration = 0; s->num_invalid = 0; s->reuse_diagonal = 0; s->n_trace = 0;
   s->num_successful = 0; s->num_unsuccessful = 0; s->sweeps = 0; s->pad0 = 0;
@@ -98,8 +110,10 @@ CLC_HD void lm_init(LmCore* s, const double* pose7, const clc_lm_options& opt) {
 }
 
 // Consumes the 28 sums of the sweep that has just evaluated s->cand and advances the minimiser until it either
-// terminates (s->done != 0) or has a new candidate in s->cand for the next sweep.
-CLC_HD void lm_update(LmCore* s, clc_lm_iteration* trace, const double* sums) {
+// terminates (s->done != 0) or has a new candidate in s->cand for the next sweep.  Trace: a clc_lm_iteration* of kTraceMax
+// rows, or TraceRows.
+template <class Trace>
+CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
   if (s->done) return;
   CLC_LM_STAMP(0);
   s->sweeps++;

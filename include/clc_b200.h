@@ -208,6 +208,37 @@ typedef struct {
  * communicator reports its own frames (its clc_shard_range); no collective. */
 int clc_frame_report(clc_problem* p, const double pose7[7], clc_frame_row* rows);
 
+/* Independent extrinsics of runs of consecutive frames (many rigs recorded into one problem, or time windows of one recording),
+ * sharing every sweep of the device-resident problem: one pass over the points per evaluation or LM iteration, whatever the
+ * number of segments.  Replaces W separate problems (clc_problem_subset of each run) and W clc_eval / clc_information /
+ * clc_solve_lm calls.
+ * A segmentation is seg_offsets[n_segments + 1] over the frames: seg_offsets[0] = 0, non-decreasing, seg_offsets[n_segments] =
+ * n_frames, n_segments >= 1.  Segment s owns frames [seg_offsets[s], seg_offsets[s + 1]), their points and their edge residuals;
+ * empty segments and segments of empty frames are valid.  poses[n_segments * 7]: one pose7 per segment.  Segment s's results
+ * are those of the same call on a fresh problem holding its frames alone (clc_problem_create of the slice, same use_loss and
+ * cauchy_a), up to the order of summation; an empty segment gets the fresh empty problem's.  A segment's results depend on its
+ * own frames only: a NaN point in one segment leaves every other segment's outputs bit-identical.  Every problem size runs on the
+ * sweep kernel K1; two calls return identical bytes.
+ * Rejected before the device is touched, with CLC_ERR_INVALID: a NULL problem, seg_offsets or poses, n_segments < 1, a
+ * seg_offsets that is not a segmentation of the problem's frames, a pose entry that is not finite.  A problem attached to a
+ * communicator fails with CLC_ERR_STATE. */
+/* clc_eval per segment: H36[n_segments * 36] (row-major 6x6) and g6[n_segments * 6] may be NULL; cost[n_segments] may not. */
+int clc_eval_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36, double* g6,
+                      double* cost);
+/* clc_information per segment (no loss, no edges): H36[n_segments * 36], b6[n_segments * 6], chi[n_segments],
+ * singular_values6[n_segments * 6], V36[n_segments * 36]; each may be NULL. */
+int clc_information_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36,
+                             double* b6, double* chi, double* singular_values6, double* V36);
+/* clc_solve_lm per segment: n_segments LM solves, each from poses[s] (overwritten with its result), advancing side by side, one
+ * shared sweep per iteration; a segment that has terminated stays as it is.  opt (NULL: defaults) holds for every segment.
+ * summaries[n_segments]: as clc_solve_lm's, except that device_ms is the time of the whole segmented solve and num_sweeps the
+ * segment's own count of sweeps that advanced it.  trace[n_segments * trace_cap]: segment s's iterations at trace[s * trace_cap],
+ * its first min(num_iterations, trace_cap) rows written; trace_cap in [0, 256], trace may be NULL when trace_cap is 0 (no trace
+ * memory is then allocated on the device).  NULL summaries, or a trace_cap outside [0, 256] or without trace, fail with
+ * CLC_ERR_INVALID. */
+int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, double* poses, const clc_lm_options* opt,
+                          clc_lm_summary* summaries, clc_lm_iteration* trace, int trace_cap);
+
 /* replaces: CamLaserCalClosedSolution(), reference src/LaseCamCalCeres.cpp:112-203.  Tlc16 row-major.
  * AtA81/Atb9 (the 9x9 normal equations) may be NULL. */
 int clc_closed_form(clc_problem* p, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
@@ -347,6 +378,10 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
 /* The same for clc_frame_report: each bracket holds the per-frame sweep and the split-frame fix-up, not the copy of the rows
  * to the host. */
 int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each);
+/* The same for one iteration of the segmented calls: each bracket holds the frame constants, the segment sweep, the split-frame
+ * fix-up and the two-level reduction into per-segment sums (clc_eval_segments without the copy to the host). */
+int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, int n, int flush_l2,
+                       float* ms_each);
 /* The gather of clc_problem_subset(src, keep): `n` times a scratch subset is prepared, its gather kernel is timed alone (CUDA
  * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
  * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
