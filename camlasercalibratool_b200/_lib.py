@@ -218,6 +218,9 @@ SIGNATURES = {
     "clc_problem_algorithmic_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_streamed_bytes": (C.c_int, [_P, c_int64_p]),
     "clc_problem_set_planar_mode": (C.c_int, [_P, C.c_int]),
+    "clc_problem_set_loss": (C.c_int, [_P, C.c_int, C.c_double]),
+    "clc_problem_get_loss": (C.c_int, [_P, C.POINTER(C.c_int), c_double_p]),
+    "clc_group_set_loss": (C.c_int, [_P, C.c_int, C.c_double]),
     "clc_debug_pack": (C.c_int, [C.c_int64, C.POINTER(c_double_p), c_int64_p, C.c_int64, C.c_int64, C.c_int, c_double_p,
                                  C.POINTER(C.c_int)]),
     "clc_debug_partition": (C.c_int, [_P, C.POINTER(C.c_int), c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int),

@@ -170,6 +170,23 @@ def _keep_mask(keep, n_frames):
     return np.ascontiguousarray(keep, dtype=np.uint8)
 
 
+# the loss kinds of set_loss (include/clc_b200.h CLC_LOSS_*)
+LOSS_KINDS = {"none": 0, "cauchy": 1, "huber": 2, "soft_l1": 3}
+
+
+def _loss_args(kind, a):
+    """(CLC_LOSS_* of a kind name, a) as clc_problem_set_loss accepts them: kind None means "none"; a finite and positive with
+    a^2 a normal double (roughly 1.5e-154 < a < 1.3e154).  ValueError for anything else."""
+    if kind is None:
+        kind = "none"
+    if not (isinstance(kind, str) and kind in LOSS_KINDS):
+        raise ValueError(f"loss kind must be None or one of {sorted(LOSS_KINDS)}, not {kind!r}")
+    a = float(a)
+    if not (a > 0.0 and np.isfinite(a) and np.isfinite(a * a) and a * a >= np.finfo(np.float64).tiny):
+        raise ValueError(f"the loss parameter a must be finite and positive with a^2 a normal double, not {a!r}")
+    return LOSS_KINDS[kind], a
+
+
 def _thresholds(max_abs_e, n_frames):
     """A scalar (every frame) or an array of shape (n_frames,) -> the float64 thresholds of the C ABI (checked before any
     device work: the library rejects a NaN or negative entry too)."""
@@ -329,6 +346,23 @@ class Problem:
     def set_planar_mode(self, mode):
         """1 = automatic (default): planar data runs the two-stream kernels; 0 = always the general kernels."""
         _lib.check(self._L.clc_problem_set_planar_mode(self._h, int(mode)), "clc_problem_set_planar_mode")
+
+    def set_loss(self, kind, a=0.05):
+        """The robust loss of every later eval, solve, frame_report, eval_segments and solve_segments (clc_problem_set_loss):
+        kind None / "none", "cauchy", "huber" or "soft_l1" -- Ceres' CauchyLoss, HuberLoss or SoftLOneLoss with parameter
+        a * s for a frame of scale s = 1/sqrt(#points), as the reference scales its CauchyLoss(0.05).  Creation sets
+        "cauchy" (use_loss=True) or "none", with a = cauchy_a.  information, closed_form and line_fit never use it; subset and
+        trim inherit it.  ValueError for a bad kind, or an a that is not finite and positive or whose square is not a normal
+        double; the loss is then unchanged."""
+        k, a = _loss_args(kind, a)
+        _lib.check(self._L.clc_problem_set_loss(self._h, k, a), "clc_problem_set_loss")
+
+    @property
+    def loss(self):
+        """(kind, a): the loss set_loss (or creation) chose; kind is "none", "cauchy", "huber" or "soft_l1"."""
+        k, a = C.c_int(), C.c_double()
+        _lib.check(self._L.clc_problem_get_loss(self._h, C.byref(k), C.byref(a)), "clc_problem_get_loss")
+        return {v: n for n, v in LOSS_KINDS.items()}[k.value], a.value
 
     def partition(self, warp_table=True):
         """The sweep kernel's static work partition for the active kernel family (test hook): dict with grid (blocks),
@@ -547,6 +581,11 @@ class Group:
         h = C.c_void_p()
         _lib.check(self._L.clc_group_subset(self._h, k.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(h)), "clc_group_subset")
         return Group(h)
+
+    def set_loss(self, kind, a=0.05):
+        """Problem.set_loss on every shard (clc_group_set_loss): the loss of every later group eval, solve and frame_report."""
+        k, a = _loss_args(kind, a)
+        _lib.check(self._L.clc_group_set_loss(self._h, k, a), "clc_group_set_loss")
 
     def trim(self, pose7, max_abs_e):
         """Problem.trim for the group (clc_group_trim), max_abs_e per frame in the global frame order: a new group on the same

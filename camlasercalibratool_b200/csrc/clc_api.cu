@@ -245,8 +245,9 @@ struct clc_problem {
   int64_t l2_bytes = 0;  // the device's L2 size
   int grid = 0;
   int64_t n_frames = 0, n_points = 0, n_points_padded = 0, n_edges = 0;
-  int use_loss = 1;
-  double cauchy_a = 0.05;
+  int loss_kind = CLC_LOSS_CAUCHY;  // clc_problem_set_loss (creation: use_loss ? CAUCHY : NONE, with a = cauchy_a)
+  double loss_a = 0.05;
+  double cauchy_a = 0.05;           // the creation's cauchy_a: clc_problem_line_fit's own Cauchy loss
   // device buffers
   double *x = nullptr, *y = nullptr, *z = nullptr;  // views into xy_block / z_block
   void *xy_block = nullptr, *z_block = nullptr;     // the allocations (x and y share one; z is created only when needed)
@@ -312,9 +313,31 @@ clc::ProblemView make_view(const clc_problem* p) {
   v.n_edges = p->n_edges;
   v.per_warp = p->per_warp;
   v.resident_chunks = p->resident_chunks;
-  v.a2 = p->cauchy_a * p->cauchy_a;
+  v.a2 = p->loss_a * p->loss_a;
   v.inv_a2 = 1.0 / v.a2;
   return v;
+}
+
+// the loss a creation descriptor asks for: CauchyLoss(cauchy_a) or none; clc_problem_set_loss changes it later
+void set_creation_loss(clc_problem* p, int use_loss, double cauchy_a) {
+  p->loss_kind = use_loss ? CLC_LOSS_CAUCHY : CLC_LOSS_NONE;
+  p->loss_a = cauchy_a;
+  p->cauchy_a = cauchy_a;
+}
+
+using SweepFn = void (*)(clc::ProblemView, clc::SweepArgs);
+
+// the sweep instantiation of a loss kind (clc::LossKind); nullptr for an unknown kind
+template <int MODE, bool LOOP = false>
+SweepFn sweep_fn(int loss, bool planar) {
+  using namespace clc;
+  switch (loss) {
+    case kLossNone: return planar ? clc_sweep_kernel<kLossNone, MODE, true, LOOP> : clc_sweep_kernel<kLossNone, MODE, false, LOOP>;
+    case kLossCauchy: return planar ? clc_sweep_kernel<kLossCauchy, MODE, true, LOOP> : clc_sweep_kernel<kLossCauchy, MODE, false, LOOP>;
+    case kLossHuber: return planar ? clc_sweep_kernel<kLossHuber, MODE, true, LOOP> : clc_sweep_kernel<kLossHuber, MODE, false, LOOP>;
+    case kLossSoftL1: return planar ? clc_sweep_kernel<kLossSoftL1, MODE, true, LOOP> : clc_sweep_kernel<kLossSoftL1, MODE, false, LOOP>;
+    default: return nullptr;
+  }
 }
 
 int set_device(const clc_problem* p) {
@@ -325,7 +348,21 @@ int set_device(const clc_problem* p) {
 // one K1 launch on the problem's stream
 // collective: the sums of this launch are to be all-reduced (in-kernel when the peer path is active)
 // kModeFrames: frame_rows / frame_slots receive the per-frame report (clc_frame_fixup_kernel finishes it)
-int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* d_pose, const int* d_done,
+// the one-cluster kernel of a loss kind (clc::LossKind): one evaluation (EVAL) or the whole LM solve; nullptr for an unknown kind
+using SmallFn = void (*)(clc::ProblemView, clc::LmState*, int, int, const double*, double*);
+template <bool EVAL>
+SmallFn small_fn(int loss) {
+  switch (loss) {
+    case clc::kLossNone: return clc::clc_small_lm_kernel<clc::kLossNone, EVAL>;
+    case clc::kLossCauchy: return clc::clc_small_lm_kernel<clc::kLossCauchy, EVAL>;
+    case clc::kLossHuber: return clc::clc_small_lm_kernel<clc::kLossHuber, EVAL>;
+    case clc::kLossSoftL1: return clc::clc_small_lm_kernel<clc::kLossSoftL1, EVAL>;
+    default: return nullptr;
+  }
+}
+
+// loss: the loss kind of the sweep (clc::LossKind)
+int launch_sweep(clc_problem* p, int mode, int loss, bool edges, const double* d_pose, const int* d_done,
                  clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false,
                  double* frame_rows = nullptr, double* frame_slots = nullptr, const double* seg_consts = nullptr) {
   clc::SweepArgs a;
@@ -336,7 +373,7 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
   a.launch_seq = p->launch_seq;
   a.pose_ll = p->pose_ll;
   a.lm = d_lm;
-  a.use_loss = loss ? 1 : 0;
+  a.use_loss = loss != clc::kLossNone ? 1 : 0;
   a.use_edges = edges ? 1 : 0;
   a.l2_hints = l2_hints ? 1 : 0;
   a.loop_sweeps = loop_sweeps;
@@ -373,9 +410,8 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
     // the per-frame report: no LM state, no L2 hints, never collective
     if (frame_rows == nullptr || frame_slots == nullptr || d_lm != nullptr || loop_sweeps > 1 || a.nranks > 1)
       return fail(CLC_ERR_INVALID, "internal: bad per-frame sweep");
-    void (*fn)(clc::ProblemView, clc::SweepArgs) =
-        loss ? (p->planar ? clc::clc_sweep_kernel<true, clc::kModeFrames, true> : clc::clc_sweep_kernel<true, clc::kModeFrames, false>)
-             : (p->planar ? clc::clc_sweep_kernel<false, clc::kModeFrames, true> : clc::clc_sweep_kernel<false, clc::kModeFrames, false>);
+    const SweepFn fn = sweep_fn<clc::kModeFrames>(loss, p->planar);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
   } else if (mode == clc::kModeSegments) {
@@ -383,29 +419,19 @@ int launch_sweep(clc_problem* p, int mode, bool loss, bool edges, const double* 
     if (frame_rows == nullptr || frame_slots == nullptr || seg_consts == nullptr || d_lm != nullptr || loop_sweeps > 1 ||
         a.nranks > 1)
       return fail(CLC_ERR_INVALID, "internal: bad segmented sweep");
-    void (*fn)(clc::ProblemView, clc::SweepArgs) =
-        loss ? (p->planar ? clc::clc_sweep_kernel<true, clc::kModeSegments, true> : clc::clc_sweep_kernel<true, clc::kModeSegments, false>)
-             : (p->planar ? clc::clc_sweep_kernel<false, clc::kModeSegments, true> : clc::clc_sweep_kernel<false, clc::kModeSegments, false>);
+    const SweepFn fn = sweep_fn<clc::kModeSegments>(loss, p->planar);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
   } else if (mode == clc::kModeClosedForm) {
-    le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeClosedForm, true>, v, a)
-                   : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeClosedForm, false>, v, a);
-  } else if (loop_sweeps > 1) {
-    // the instantiations that loop the LM inside the kernel (one launch per solve)
-    if (d_lm == nullptr) return fail(CLC_ERR_INVALID, "internal: looping sweep without an LM state");
-    if (loss)
-      le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<true, clc::kModeLM, true, true>, v, a)
-                     : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<true, clc::kModeLM, false, true>, v, a);
-    else
-      le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeLM, true, true>, v, a)
-                     : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeLM, false, true>, v, a);
-  } else if (loss) {
-    le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<true, clc::kModeLM, true>, v, a)
-                   : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<true, clc::kModeLM, false>, v, a);
+    le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<clc::kLossNone, clc::kModeClosedForm, true>, v, a)
+                   : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<clc::kLossNone, clc::kModeClosedForm, false>, v, a);
   } else {
-    le = p->planar ? cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeLM, true>, v, a)
-                   : cudaLaunchKernelEx(&cfg, clc::clc_sweep_kernel<false, clc::kModeLM, false>, v, a);
+    // loop_sweeps > 1: the instantiations that loop the LM inside the kernel (one launch per solve)
+    if (loop_sweeps > 1 && d_lm == nullptr) return fail(CLC_ERR_INVALID, "internal: looping sweep without an LM state");
+    const SweepFn fn = loop_sweeps > 1 ? sweep_fn<clc::kModeLM, true>(loss, p->planar) : sweep_fn<clc::kModeLM>(loss, p->planar);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    le = cudaLaunchKernelEx(&cfg, fn, v, a);
   }
   if (le != cudaSuccess) return fail(CLC_ERR_CUDA, std::string("sweep launch: ") + cudaGetErrorString(le));
   CLC_LAUNCH_CHECK();
@@ -508,13 +534,17 @@ int finish_create(clc_problem* p) {
   }
   if (blocks_per_sm == 0) {
     int occ = 0, occ_min = 1 << 30;
-    const void* variants[] = {
-        (const void*)clc::clc_sweep_kernel<true, clc::kModeLM, false>,         (const void*)clc::clc_sweep_kernel<true, clc::kModeLM, true>,
-        (const void*)clc::clc_sweep_kernel<false, clc::kModeLM, false>,        (const void*)clc::clc_sweep_kernel<false, clc::kModeLM, true>,
-        (const void*)clc::clc_sweep_kernel<false, clc::kModeClosedForm, false>, (const void*)clc::clc_sweep_kernel<false, clc::kModeClosedForm, true>,
-        (const void*)clc::clc_sweep_kernel<true, clc::kModeLM, false, true>,   (const void*)clc::clc_sweep_kernel<true, clc::kModeLM, true, true>,
-        (const void*)clc::clc_sweep_kernel<false, clc::kModeLM, false, true>,  (const void*)clc::clc_sweep_kernel<false, clc::kModeLM, true, true>};
-    for (int v = 0; v < 10; ++v) {
+    // every loss kind's LM instantiations (one launch per iteration, and looping), then the closed form; planar at odd entries
+    std::vector<const void*> variants;
+    for (int loss = clc::kLossNone; loss <= clc::kLossSoftL1; ++loss) {
+      variants.push_back((const void*)sweep_fn<clc::kModeLM>(loss, false));
+      variants.push_back((const void*)sweep_fn<clc::kModeLM>(loss, true));
+      variants.push_back((const void*)sweep_fn<clc::kModeLM, true>(loss, false));
+      variants.push_back((const void*)sweep_fn<clc::kModeLM, true>(loss, true));
+    }
+    variants.push_back((const void*)clc::clc_sweep_kernel<clc::kLossNone, clc::kModeClosedForm, false>);
+    variants.push_back((const void*)clc::clc_sweep_kernel<clc::kLossNone, clc::kModeClosedForm, true>);
+    for (int v = 0; v < (int)variants.size(); ++v) {
       const void* fn = variants[v];
       const int smem = clc::dyn_smem_bytes((v & 1) != 0);  // odd entries are the planar instantiations
       CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -772,8 +802,7 @@ int create_shell(clc_problem** out, const HostSource& src, int use_loss, double 
   p->n_frames = N;
   p->n_points = P;
   p->n_edges = src.edge_points ? 2 * N : 0;
-  p->use_loss = use_loss;
-  p->cauchy_a = cauchy_a;
+  set_creation_loss(p, use_loss, cauchy_a);
   auto body = [&]() -> int {
     // the z stream is created only if a z != 0 turns up (pack path) -- a pinned flat source is laid out by the device
     // kernel that also checks planarity, which needs it from the start
@@ -891,8 +920,7 @@ int clc_problem_create_synthetic(clc_problem** out, const clc_synthetic_desc* d)
   p->n_frames = N;
   p->n_points = N * d->beams;
   p->n_edges = d->with_edges ? 2 * N : 0;
-  p->use_loss = d->use_loss;
-  p->cauchy_a = d->cauchy_a;
+  set_creation_loss(p, d->use_loss, d->cauchy_a);
   auto body = [&]() -> int {
     // the simulated laser is two-dimensional (calibr_simulation.cpp:82,88): planar by construction, no z stream
     int rc2 = alloc_points(p, /*with_z=*/false);
@@ -988,6 +1016,32 @@ int clc_problem_set_planar_mode(clc_problem* p, int mode) {
   return partition(p);
 }
 
+namespace {
+int check_loss(int kind, double a) {
+  if (kind < CLC_LOSS_NONE || kind > CLC_LOSS_SOFT_L1) return fail(CLC_ERR_INVALID, "unknown loss kind");
+  // a^2 normal: a is finite and positive, 1/a^2 is finite, and sqrt(a * a) == a (the Huber kernels take a from a^2)
+  if (!(a > 0.0) || !std::isnormal(a * a)) return fail(CLC_ERR_INVALID, "the loss parameter a must be finite, positive, with a^2 a normal double");
+  return CLC_OK;
+}
+}  // namespace
+
+int clc_problem_set_loss(clc_problem* p, int kind, double a) {
+  if (!p) return fail(CLC_ERR_INVALID, "NULL problem");
+  const int rc = check_loss(kind, a);  // before the problem is touched
+  if (rc != CLC_OK) return rc;
+  // launches already enqueued took the old loss by value (ProblemView): no synchronisation needed
+  p->loss_kind = kind;
+  p->loss_a = a;
+  return CLC_OK;
+}
+
+int clc_problem_get_loss(const clc_problem* p, int* kind, double* a) {
+  if (!p || !kind || !a) return fail(CLC_ERR_INVALID, "NULL argument");
+  *kind = p->loss_kind;
+  *a = p->loss_a;
+  return CLC_OK;
+}
+
 int clc_problem_download(const clc_problem* p, double* frame_pose, int64_t* offsets, double* points,
                          double* edge_points, double* planes) {
   if (!p) return fail(CLC_ERR_INVALID, "NULL problem");
@@ -1036,7 +1090,8 @@ static bool sweep_loops_in_kernel(const clc_problem* p) {
 // which case K3 runs it as its own launch.
 static bool fused_lm_update(const clc_problem* p) { return p->nranks <= 1 || p->allreduce_mode == 1; }
 
-static int eval_enqueue(clc_problem* p, const double pose7[7], bool loss, bool edges, int mode, int count) {
+// loss: the loss kind (clc::LossKind)
+static int eval_enqueue(clc_problem* p, const double pose7[7], int loss, bool edges, int mode, int count) {
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   double* h_pose = p->pinned->pose;  // pinned: the copy below is truly asynchronous
@@ -1052,10 +1107,9 @@ static int eval_enqueue(clc_problem* p, const double pose7[7], bool loss, bool e
   if (mode == clc::kModeLM && small_kernel_serves(p, with_edges)) {
     // a small problem: one evaluation by the one-cluster kernel (clc_small.cuh)
     const clc::ProblemView v = make_view(p);
-    if (loss)
-      clc::clc_small_lm_kernel<true, true><<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, nullptr, 1, with_edges ? 1 : 0, p->pose, p->sums);
-    else
-      clc::clc_small_lm_kernel<false, true><<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, nullptr, 1, with_edges ? 1 : 0, p->pose, p->sums);
+    const SmallFn fn = small_fn<true>(loss);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    fn<<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, nullptr, 1, with_edges ? 1 : 0, p->pose, p->sums);
     CLC_LAUNCH_CHECK();
   } else {
     rc = launch_sweep(p, mode, loss, edges, p->pose, nullptr, nullptr);
@@ -1081,9 +1135,9 @@ static int eval_all(clc_problem* const* ps, int n, const double pose7[7], int wh
   for (int g = 0; g < n; ++g) {
     clc_problem* p = ps[g];
     int rc;
-    if (which == 0) rc = eval_enqueue(p, pose7, p->use_loss != 0, p->n_edges > 0, clc::kModeLM, clc::kNumSums);
-    else if (which == 1) rc = eval_enqueue(p, pose7, false, false, clc::kModeLM, clc::kNumSums);  // reference :318-381: no loss, no edges
-    else rc = eval_enqueue(p, nullptr, false, false, clc::kModeClosedForm, clc::kMaxOut);
+    if (which == 0) rc = eval_enqueue(p, pose7, p->loss_kind, p->n_edges > 0, clc::kModeLM, clc::kNumSums);
+    else if (which == 1) rc = eval_enqueue(p, pose7, clc::kLossNone, false, clc::kModeLM, clc::kNumSums);  // reference :318-381: no loss, no edges
+    else rc = eval_enqueue(p, nullptr, clc::kLossNone, false, clc::kModeClosedForm, clc::kMaxOut);
     if (rc != CLC_OK && first_rc == CLC_OK) first_rc = rc;
   }
   for (int g = 0; g < n; ++g) {
@@ -1239,17 +1293,20 @@ void frame_report_free(clc_problem* p, FrameReportBuffers* b) {
 
 // the report at the pose in p->pose: the per-frame sweep, then the fix-up of split and empty frames
 int frame_report_launch(clc_problem* p, const FrameReportBuffers& b) {
-  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
   int rc = launch_sweep(p, clc::kModeFrames, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false, /*pdl=*/false,
                         /*loop_sweeps=*/1, /*l2_hints=*/false, b.rows, b.slots);
   if (rc != CLC_OK) return rc;
   const int threads = 256;
   const unsigned blocks = (unsigned)((p->n_frames + threads - 1) / threads);
   const clc::ProblemView v = make_view(p);
-  if (loss)
-    clc::clc_frame_fixup_kernel<true><<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
-  else
-    clc::clc_frame_fixup_kernel<false><<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
+  void (*fixup)(clc::ProblemView, const double*, int, const double*, double*) =
+      loss == clc::kLossCauchy  ? clc::clc_frame_fixup_kernel<clc::kLossCauchy>
+      : loss == clc::kLossHuber ? clc::clc_frame_fixup_kernel<clc::kLossHuber>
+      : loss == clc::kLossSoftL1 ? clc::clc_frame_fixup_kernel<clc::kLossSoftL1>
+                                 : clc::clc_frame_fixup_kernel<clc::kLossNone>;
+  fixup<<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
   CLC_LAUNCH_CHECK();
   return CLC_OK;
 }
@@ -1305,7 +1362,8 @@ struct SolveCtx {
   clc_lm_options opt;
   int max_sweeps = 0;
   int launched = 0;
-  bool fused_update = true, loss = true, edges = false;
+  bool fused_update = true, edges = false;
+  int loss = clc::kLossCauchy;  // clc::LossKind
 };
 
 // L2 residency across LM iterations: every iteration re-reads the same coordinate arrays.  When they are not much larger than
@@ -1355,7 +1413,7 @@ int solve_begin(clc_problem* p, const double pose7[7], const clc_lm_options& opt
   CLC_CUDA(cudaMemcpyAsync(&p->lm->core, &p->h_lm->core, sizeof(clc::LmCore), cudaMemcpyHostToDevice, p->stream));
   CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
   ctx->fused_update = fused_lm_update(p);
-  ctx->loss = p->use_loss != 0;
+  ctx->loss = p->loss_kind;
   ctx->edges = p->n_edges > 0;
   // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps
   ctx->max_sweeps = opt.max_num_iterations + 2;
@@ -1469,10 +1527,9 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
     rc = set_device(p);
     if (rc != CLC_OK) return rc;
     const clc::ProblemView v = make_view(p);
-    if (ctx[0].loss)
-      clc::clc_small_lm_kernel<true><<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, p->lm, max_sweeps, ctx[0].edges ? 1 : 0, nullptr, nullptr);
-    else
-      clc::clc_small_lm_kernel<false><<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, p->lm, max_sweeps, ctx[0].edges ? 1 : 0, nullptr, nullptr);
+    const SmallFn fn = small_fn<false>(ctx[0].loss);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    fn<<<clc::kSmallCluster, clc::kSmallThreads, 0, p->stream>>>(v, p->lm, max_sweeps, ctx[0].edges ? 1 : 0, nullptr, nullptr);
     CLC_LAUNCH_CHECK();
     launched = max_sweeps;
   }
@@ -1615,7 +1672,7 @@ int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, Segm
 
 // One shared sweep of every segment: pose s at poses[s * pose_stride] on the device.  sums: [W * kNumSums] or nullptr; cores:
 // the solve's LmCores (lm_update runs on every segment that has not terminated), with its trace, counters and `done` flag.
-int segments_iteration(const SegmentRun& r, bool loss, bool edges, const double* poses, int64_t pose_stride, double* sums,
+int segments_iteration(const SegmentRun& r, int loss, bool edges, const double* poses, int64_t pose_stride, double* sums,
                        clc::LmCore* cores, clc_lm_iteration* trace, int trace_cap, int* counters) {
   clc_problem* p = r.p;
   int* done = counters != nullptr ? counters + 1 : nullptr;  // raised when every segment has terminated
@@ -1630,10 +1687,12 @@ int segments_iteration(const SegmentRun& r, bool loss, bool edges, const double*
     int rc = launch_sweep(p, clc::kModeSegments, loss, with_edges, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
                           /*loop_sweeps=*/1, /*l2_hints=*/false, r.raw, r.slots, r.consts);
     if (rc != CLC_OK) return rc;
-    if (loss)
-      clc::clc_segment_fixup_kernel<true><<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
-    else
-      clc::clc_segment_fixup_kernel<false><<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
+    void (*fixup)(clc::ProblemView, const double*, int, const int*, const double*, const double*, double*) =
+        loss == clc::kLossCauchy  ? clc::clc_segment_fixup_kernel<clc::kLossCauchy>
+        : loss == clc::kLossHuber ? clc::clc_segment_fixup_kernel<clc::kLossHuber>
+        : loss == clc::kLossSoftL1 ? clc::clc_segment_fixup_kernel<clc::kLossSoftL1>
+                                   : clc::clc_segment_fixup_kernel<clc::kLossNone>;
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
     CLC_LAUNCH_CHECK();
   }
   if (r.n_chunks > 0) {
@@ -1659,7 +1718,8 @@ int eval_segments_run(clc_problem* p, int64_t W, const int64_t* seg_offsets, con
   if ((rc = seg_alloc(p, &r.poses, (size_t)W * 7)) != CLC_OK || (rc = seg_alloc(p, &r.sums, (size_t)W * clc::kNumSums)) != CLC_OK)
     return rc;
   CLC_CUDA(cudaMemcpyAsync(r.poses, poses, sizeof(double) * 7 * (size_t)W, cudaMemcpyHostToDevice, p->stream));
-  const bool loss = which == 0 && p->use_loss != 0, edges = which == 0 && p->n_edges > 0;
+  const int loss = which == 0 ? p->loss_kind : clc::kLossNone;
+  const bool edges = which == 0 && p->n_edges > 0;
   rc = segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
   if (rc != CLC_OK) return rc;
   sums->resize((size_t)W * clc::kNumSums);
@@ -1716,7 +1776,8 @@ int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg
   if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
   if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
   CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
-  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
   // the candidate pose of segment s: cores[s].cand, sizeof(LmCore) / 8 doubles apart
   const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.cores) + offsetof(clc::LmCore, cand));
   const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
@@ -2321,6 +2382,18 @@ int clc_group_problem(clc_group* g, int index, clc_problem** out) {
   return CLC_OK;
 }
 
+int clc_group_set_loss(clc_group* g, int kind, double a) {
+  if (!g) return fail(CLC_ERR_INVALID, "NULL group");
+  const int rc = check_loss(kind, a);  // before the group is touched
+  if (rc != CLC_OK) return rc;
+  if (g->problems.empty()) return fail(CLC_ERR_INVALID, "empty group");
+  for (clc_problem* p : g->problems) {
+    p->loss_kind = kind;
+    p->loss_a = a;
+  }
+  return CLC_OK;
+}
+
 int clc_group_eval(clc_group* g, const double pose7[7], double H36[36], double g6[6], double* cost) {
   if (!g || g->problems.empty()) return fail(CLC_ERR_INVALID, "NULL group");
   int rc = eval_all(g->problems.data(), (int)g->problems.size(), pose7, 0);
@@ -2385,9 +2458,10 @@ void subset_release(std::vector<SubsetShard>& shards) {
   shards.clear();
 }
 
-// The shell of a destination shard: sizes, the source's loss, point arrays with zeroed padding, per-frame arrays, offsets.
+// The shell of a destination shard: sizes, the loss of `src` (kind, a and the line fit's cauchy_a), point arrays with zeroed
+// padding, per-frame arrays, offsets.
 int subset_shell(clc_problem** out, int device, int64_t N, int64_t P, const int64_t* offsets, bool with_z, bool edges,
-                 bool true_poses, int use_loss, double cauchy_a) {
+                 bool true_poses, const clc_problem* src) {
   clc_problem* p = new clc_problem();
   *out = p;
   int rc = init_device(p, device);
@@ -2395,8 +2469,9 @@ int subset_shell(clc_problem** out, int device, int64_t N, int64_t P, const int6
   p->n_frames = N;
   p->n_points = P;
   p->n_edges = edges ? 2 * N : 0;
-  p->use_loss = use_loss;
-  p->cauchy_a = cauchy_a;
+  p->loss_kind = src->loss_kind;
+  p->loss_a = src->loss_a;
+  p->cauchy_a = src->cauchy_a;
   rc = alloc_points(p, with_z);
   if (rc != CLC_OK) return rc;
   CLC_CUDA(cudaMallocAsync(&p->frame_pose, sizeof(double) * 7 * std::max<int64_t>(N, 1), p->stream));
@@ -2464,8 +2539,7 @@ int subset_prepare(const std::vector<clc_problem*>& src, const uint8_t* keep, co
       work.push_back(r);
     }
     work.insert(work.end(), frame_src.begin(), frame_src.end());
-    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]->use_loss,
-                          src[0]->cauchy_a);
+    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]);
     if (rc != CLC_OK) return rc;
     clc_problem* p = sh.p;
     CLC_CUDA(cudaMallocAsync(&sh.d_work, sizeof(int64_t) * std::max<size_t>(work.size(), 1), p->stream));
@@ -2779,8 +2853,7 @@ int trim_prepare(const std::vector<clc_problem*>& src, const std::vector<TrimMar
       const int64_t k0 = plan.tile_prefix[base.src_tile_begin[s]], k1 = plan.tile_prefix[base.src_tile_begin[s + 1]];
       sh.gathers_z = sh.gathers_z || (base.src[s].z != nullptr && std::max(k0, p0) < std::min(k1, p0 + P));
     }
-    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]->use_loss,
-                          src[0]->cauchy_a);
+    int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]);
     if (rc != CLC_OK) return rc;
     clc_problem* p = sh.p;
     const int64_t t_begin = plan.tile_begin[d], n_tiles = plan.tile_begin[d + 1] - t_begin;
@@ -3050,7 +3123,8 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
   if (rc != CLC_OK) return rc;
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
-  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
   return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
     return launch_sweep(p, clc::kModeLM, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false);
   });
@@ -3070,7 +3144,8 @@ int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_of
   int flush_smem = 0;
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
   if (rc != CLC_OK) return rc;
-  const bool loss = p->use_loss != 0, edges = p->n_edges > 0;
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
   return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
     return segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
   });
@@ -3175,7 +3250,7 @@ int clc_debug_sweep_timing(clc_problem* p, const double pose7[7], int with_lm, i
   clc::lm_init(&p->h_lm->core, pose7, opt);
   CLC_CUDA(cudaMemcpyAsync(p->lm, p->h_lm, sizeof(clc::LmState), cudaMemcpyHostToDevice, p->stream));
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
-  rc = launch_sweep(p, clc::kModeLM, p->use_loss != 0, p->n_edges > 0, p->pose, nullptr, with_lm ? p->lm : nullptr, /*collective=*/false);
+  rc = launch_sweep(p, clc::kModeLM, p->loss_kind, p->n_edges > 0, p->pose, nullptr, with_lm ? p->lm : nullptr, /*collective=*/false);
   cudaError_t e = cudaMemcpyAsync(stamps, p->timing, bytes, cudaMemcpyDeviceToHost, p->stream);
   if (e == cudaSuccess && warp_stamps)
     e = cudaMemcpyAsync(warp_stamps, p->timing + 8 * (size_t)p->grid, wbytes, cudaMemcpyDeviceToHost, p->stream);

@@ -5,18 +5,51 @@
 //   raw distance        e_j = n^T(R p_j + t) + d = m.p_j + c
 //   residual            r_j = s e_j,  s = 1/sqrt(#points of the frame)      (reference src/LaseCamCalCeres.cpp:239-240,:48)
 //   Jacobian (1x6)      J_j = s [ n^T , (p_j x m)^T ]                         (:54-60:  n^T(-R [p]x) = (p x m)^T)
-//   Cauchy weight       w_j = rho'(r_j^2) = 1 / (1 + e_j^2 / a^2), a = 0.05  (:249; the scale s cancels)
+//   robust weight       w_j = rho'(r_j^2), e.g. Cauchy 1 / (1 + e_j^2 / a^2), a = 0.05  (:249; the scale s cancels)
 // J_t = n is constant over the frame and J_theta = p x m = -[m]x p is linear in p, so everything the LM step
 // needs is a linear image of the weighted moments  S0 = sum w, S1 = sum w p, S2 = sum w p p^T:
 //   sum w J^T J = s^2 [ S0 n n^T        n (S1 x m)^T      ]      sum w e J^T = s^2 [ (m.S1 + c S0) n      ]
 //                     [ .               [m]x S2 [m]x^T    ]                        [ (S2 m + c S1) x m    ]
 // and the robust cost is 1/2 a^2 s^2 sum log(1 + e^2/a^2) = 1/2 a^2 s^2 log(prod (1 + e^2/a^2)).
 // The kernel therefore keeps 10 moment accumulators + a running product per lane instead of 28 sums.
+// This holds for every loss with rho'' <= 0 (LossKind below): Ceres' Corrector then scales r and J by sqrt(rho'), so
+// sum w J^T J and sum w e J^T are the same linear images of the moments -- only w and the cost term change.
 #pragma once
 
 #include "clc_math.cuh"
 
 namespace clc {
+
+// Robust losses (include/clc_b200.h CLC_LOSS_*).  A frame with scale s uses loss parameter a s on r = s e (reference :249), so
+// with z = e^2 / a^2 the scale cancels from the weight; the frame's cost is 1/2 s^2 sum rho~(e), and a^2 times that for Cauchy:
+//   kind      w = rho'                       rho~(e)
+//   none      1                              e^2
+//   Cauchy    1 / (1 + z)                    log(1 + z)
+//   Huber     1 if |e| <= a, else a / |e|    e^2 if |e| <= a, else 2 a |e| - a^2
+//   soft-L1   1 / sqrt(1 + z)                2 e^2 / (1 + sqrt(1 + z))   (Ceres' 2 a^2 (sqrt(1 + z) - 1) without cancellation)
+// Every kind has rho'' <= 0 (Ceres' simple corrector branch).  |e| == a is a Huber inlier.
+enum LossKind { kLossNone = 0, kLossCauchy = 1, kLossHuber = 2, kLossSoftL1 = 3 };
+
+// w and rho~ of one residual (the single-residual paths: the one-cluster kernel, the edge residuals).  a2 = a^2, inv_a2 = 1/a2.
+// Huber takes a = sqrt(a2), which is exact: sqrt(fl(a * a)) == a in binary floating point when a^2 is normal.
+CLC_HD void loss_weight(int kind, double e, double a2, double inv_a2, double* w, double* cost_term) {
+  if (kind == kLossCauchy) {
+    const double u = fma(e * inv_a2, e, 1.0);
+    *w = 1.0 / u;
+    *cost_term = log(u);
+  } else if (kind == kLossHuber) {
+    const double a = sqrt(a2), ae = fabs(e);
+    *w = ae <= a ? 1.0 : a / ae;
+    *cost_term = ae <= a ? e * e : fma(2.0 * a, ae, -a2);
+  } else if (kind == kLossSoftL1) {
+    const double t = sqrt(fma(e * inv_a2, e, 1.0));
+    *w = 1.0 / t;
+    *cost_term = 2.0 * e * e / (1.0 + t);
+  } else {
+    *w = 1.0;
+    *cost_term = e * e;
+  }
+}
 
 // Pose-dependent constants shared by all frames of one sweep.
 struct PoseConsts {
@@ -47,10 +80,10 @@ CLC_HD double point_distance(const double* m, double c, double x, double y, doub
 // Moments layout: S[0]=S0, S[1..3]=S1 (x,y,z), S[4..9]=S2 (xx,xy,xz,yy,yz,zz).
 // Adds the piece's contribution to out[28] = 21 upper-tri H (row-major, i<=j), 6 g, 1 cost.
 //   s2        = 1/(#points of the whole frame)
-//   cost_term = sum log(1 + e^2/a^2) over the piece when the loss is on, sum e^2 otherwise (accumulated directly:
-//               deriving it from the moments would cancel catastrophically near the optimum)
-//   a2        = cauchy_a^2
-CLC_HD void expand_lm(const double* plane, const double* m, double c, double s2, const double* S, bool use_loss,
+//   cost_term = sum rho~(e) over the piece (LossKind; accumulated directly: deriving it from the moments would cancel
+//               catastrophically near the optimum)
+//   loss      = LossKind, a2 = a^2
+CLC_HD void expand_lm(const double* plane, const double* m, double c, double s2, const double* S, int loss,
                       double cost_term, double a2, double* out) {
   const double n[3] = {plane[0], plane[1], plane[2]};
   const double S0 = S[0];
@@ -91,26 +124,30 @@ CLC_HD void expand_lm(const double* plane, const double* m, double c, double s2,
   // g
   out[21] += sn[0] * E0; out[22] += sn[1] * E0; out[23] += sn[2] * E0;
   out[24] += s2 * vxm[0]; out[25] += s2 * vxm[1]; out[26] += s2 * vxm[2];
-  // cost: 1/2 a^2 s^2 sum log(1 + e^2/a^2) with the loss, 1/2 s^2 sum e^2 without
-  out[27] += use_loss ? 0.5 * a2 * s2 * cost_term : 0.5 * s2 * cost_term;
+  // cost: 1/2 a^2 s^2 sum log(1 + e^2/a^2) with the Cauchy loss, 1/2 s^2 sum rho~(e) otherwise
+  out[27] += loss == kLossCauchy ? 0.5 * a2 * s2 * cost_term : 0.5 * s2 * cost_term;
 }
 
 // One residual added DIRECTLY to acc[28] (21 upper-tri H, 6 g, cost) -- what the one-cluster kernel for small problems does
 // (clc_small.cuh): no moments, the plain PointInPlaneFactor arithmetic of reference src/LaseCamCalCeres.cpp:43-66 with the
 // Cauchy correction of :249.  plane = (n, d); (x, y, z) the laser point; s2 = 1/#points of the frame (the squared scale of
-// :239-240); a2 = cauchy_a^2, inv_a2 = 1/a2.  J = s [n, p x m] with m = R^T n; w = rho' = 1/(1 + e^2/a^2).
-CLC_HD void accumulate_residual(const PoseConsts& pc, const double* plane, double x, double y, double z, double s2, bool use_loss,
+// :239-240); loss = LossKind, a2 = a^2, inv_a2 = 1/a2.  J = s [n, p x m] with m = R^T n; w = rho' (loss_weight).
+CLC_HD void accumulate_residual(const PoseConsts& pc, const double* plane, double x, double y, double z, double s2, int loss,
                                 double a2, double inv_a2, double* acc) {
   double m[3], c;
   frame_consts(pc, plane, m, &c);
   const double e = fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
   double w = 1.0, cost;
-  if (use_loss) {
+  if (loss == kLossCauchy) {
     const double u = fma(e * inv_a2, e, 1.0);
     w = 1.0 / u;
     cost = 0.5 * a2 * s2 * log(u);
-  } else {
+  } else if (loss == kLossNone) {
     cost = 0.5 * s2 * e * e;
+  } else {
+    double t;
+    loss_weight(loss, e, a2, inv_a2, &w, &t);
+    cost = 0.5 * s2 * t;
   }
   const double J[6] = {plane[0], plane[1], plane[2], y * m[2] - z * m[1], z * m[0] - x * m[2], x * m[1] - y * m[0]};
   const double ws = w * s2;
@@ -133,27 +170,23 @@ CLC_HD void accumulate_residual(const PoseConsts& pc, const double* plane, doubl
 // One board-edge residual (plane = an edge plane, pt = its edge point) expanded through its moments into out[28], as the edge
 // tail of the sweep kernel does; returns the raw distance e.  s2 = 1/#points of the frame.
 // m, c: the edge plane's constants at the pose (frame_consts).
-CLC_HD double edge_residual_at(const double* plane, const double* m, double c, const double* pt, double s2, bool use_loss,
+CLC_HD double edge_residual_at(const double* plane, const double* m, double c, const double* pt, double s2, int loss,
                                double a2, double inv_a2, double* out) {
   const double x = pt[0], y = pt[1], z = pt[2];
   const double e = fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
-  double w = 1.0, cost_term = e * e;
-  if (use_loss) {
-    const double u = fma(e * inv_a2, e, 1.0);
-    w = 1.0 / u;
-    cost_term = log(u);
-  }
+  double w, cost_term;
+  loss_weight(loss, e, a2, inv_a2, &w, &cost_term);
   const double S[10] = {w, w * x, w * y, w * z, w * x * x, w * x * y, w * x * z, w * y * y, w * y * z, w * z * z};
-  expand_lm(plane, m, c, s2, S, use_loss, cost_term, a2, out);
+  expand_lm(plane, m, c, s2, S, loss, cost_term, a2, out);
   return e;
 }
 
 // edge_residual_at with m, c = frame_consts(pc, plane)
-CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const double* pt, double s2, bool use_loss, double a2,
+CLC_HD double edge_residual(const PoseConsts& pc, const double* plane, const double* pt, double s2, int loss, double a2,
                             double inv_a2, double* out) {
   double m[3], c;
   frame_consts(pc, plane, m, &c);
-  return edge_residual_at(plane, m, c, pt, s2, use_loss, a2, inv_a2, out);
+  return edge_residual_at(plane, m, c, pt, s2, loss, a2, inv_a2, out);
 }
 
 // Closed-form initialisation (reference src/LaseCamCalCeres.cpp:144-161): row A_k = n (x) (x, y, 1), b_k = -d, so

@@ -79,8 +79,8 @@ __host__ __device__ constexpr int frames_smem_bytes(bool planar) {
 // equations go to a row of their own instead of being summed
 // kModeSegments: independent solves over runs of frames (clc_*_segments) -- every frame's raw moments at its segment's pose go
 // to a row of their own (clc_segment_fixup_kernel expands them); the frame constants m, c come from SweepArgs::seg_consts.
-// A raw row: 10 moments, the cost (loss: product of (1 + e^2/a^2) with its exponent taken out; no loss: sum e^2) and that
-// exponent -- the layout of the first 12 doubles of a split-frame slot.
+// A raw row: 10 moments, the cost (Cauchy: product of (1 + e^2/a^2) with its exponent taken out; other kinds: sum rho~(e),
+// clc_expand.cuh) and that exponent -- the layout of the first 12 doubles of a split-frame slot.
 constexpr int kSegRawDoubles = 12;
 enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3 };
 
@@ -99,8 +99,8 @@ struct ProblemView {
   int64_t n_edges;            // 2 * n_frames or 0
   int64_t per_warp;           // points per warp (multiple of the kernel family's stage size)
   int resident_chunks;        // LM solves: the last resident_chunks stages of every warp's range are kept in L2 (clc_l2_plan.h)
-  double inv_a2;              // 1 / cauchy_a^2
-  double a2;                  // cauchy_a^2
+  double inv_a2;              // 1 / a^2 of the problem's loss
+  double a2;                  // a^2
 };
 
 struct SweepArgs {
@@ -283,14 +283,14 @@ __device__ __forceinline__ void warp_transpose_sum_regs(double* v, int lane) {
 // Per-lane streaming accumulators of one piece.
 struct Moments {
   double S0, Sx, Sy, Sz, Sxx, Sxy, Sxz, Syy, Syz, Szz;
-  double prod;  // loss on: running product of (1 + e^2/a^2), mantissa kept in [1,2); loss off: running sum of e^2
+  double prod;  // Cauchy: running product of (1 + e^2/a^2), mantissa kept in [1,2); other kinds: running sum of rho~(e)
   int esum;     // exponent taken out of prod
 };
 
-template <bool LOSS>
+template <int LOSS>
 __device__ __forceinline__ void moments_clear(Moments& a) {
   a.S0 = a.Sx = a.Sy = a.Sz = a.Sxx = a.Sxy = a.Sxz = a.Syy = a.Syz = a.Szz = 0.0;
-  a.prod = LOSS ? 1.0 : 0.0;
+  a.prod = LOSS == kLossCauchy ? 1.0 : 0.0;
   a.esum = 0;
 }
 
@@ -310,14 +310,47 @@ __device__ __forceinline__ void accumulate(Moments& a, double w, double x, doubl
   }
 }
 
-// Two points (one LDG.128 per coordinate array).  v0/v1: validity of the two points.
-template <bool LOSS, bool COST, bool PLANAR>
+// Two points (one LDG.128 per coordinate array).  v0/v1: validity of the two points.  LOSS: LossKind (clc_expand.cuh); COST:
+// the no-loss kind also sums e^2 (the other kinds always sum their cost term).  a: the loss parameter (Huber only), a2 = a^2.
+template <int LOSS, bool COST, bool PLANAR>
 __device__ __forceinline__ void process2(Moments& a, const double2 X, const double2 Y, const double2 Z, bool v0,
-                                         bool v1, double m0, double m1, double m2, double c, double inv_a2) {
+                                         bool v1, double m0, double m1, double m2, double c, double inv_a2, double ha = 0.0,
+                                         double a2 = 0.0) {
   // fma(m2, 0, c) == c exactly for finite m2, so the planar form rounds like the general one
   const double e0 = fma(m0, X.x, fma(m1, Y.x, PLANAR ? c : fma(m2, Z.x, c)));
   const double e1 = fma(m0, X.y, fma(m1, Y.y, PLANAR ? c : fma(m2, Z.y, c)));
-  if (LOSS) {
+  if (LOSS == kLossHuber) {
+    // w = a / max(|e|, a): one reciprocal of the product of the two denominators serves both weights (a NaN e stays NaN)
+    const double ae0 = fabs(e0), ae1 = fabs(e1);
+    double d0 = ae0 < ha ? ha : ae0, d1 = ae1 < ha ? ha : ae1;
+    d0 = v0 ? d0 : ha;
+    d1 = v1 ? d1 : ha;
+    const double ar = ha * rcp_pos(d0 * d1);
+    double w0 = ar * d1, w1 = ar * d0;
+    w0 = v0 ? w0 : 0.0;
+    w1 = v1 ? w1 : 0.0;
+    // rho~ = e^2 inside a, 2 a |e| - a^2 outside: summed directly, like e^2 without a loss
+    const double r0 = ae0 <= ha ? e0 * e0 : fma(2.0 * ha, ae0, -a2);
+    const double r1 = ae1 <= ha ? e1 * e1 : fma(2.0 * ha, ae1, -a2);
+    a.prod += v0 ? r0 : 0.0;
+    a.prod += v1 ? r1 : 0.0;
+    accumulate<PLANAR>(a, w0, X.x, Y.x, Z.x);
+    accumulate<PLANAR>(a, w1, X.y, Y.y, Z.y);
+  } else if (LOSS == kLossSoftL1) {
+    // w = 1/sqrt(u), u = 1 + e^2/a^2; rho~ = 2 e^2 / (1 + sqrt(u)) with sqrt(u) = u w -- one reciprocal for both points
+    double u0 = fma(e0 * inv_a2, e0, 1.0);
+    double u1 = fma(e1 * inv_a2, e1, 1.0);
+    u0 = v0 ? u0 : 1.0;
+    u1 = v1 ? u1 : 1.0;
+    const double y0 = rsqrt(u0), y1 = rsqrt(u1);
+    const double t0 = fma(u0, y0, 1.0), t1 = fma(u1, y1, 1.0);
+    const double r = rcp_pos(t0 * t1);
+    const double r0 = (2.0 * e0) * e0 * (r * t1), r1 = (2.0 * e1) * e1 * (r * t0);
+    a.prod += v0 ? r0 : 0.0;
+    a.prod += v1 ? r1 : 0.0;
+    accumulate<PLANAR>(a, v0 ? y0 : 0.0, X.x, Y.x, Z.x);
+    accumulate<PLANAR>(a, v1 ? y1 : 0.0, X.y, Y.y, Z.y);
+  } else if (LOSS == kLossCauchy) {
     double u0 = fma(e0 * inv_a2, e0, 1.0);
     double u1 = fma(e1 * inv_a2, e1, 1.0);
     u0 = v0 ? u0 : 1.0;
@@ -375,7 +408,7 @@ __device__ __forceinline__ void frame_sums2(FrameSums& s, const double2 X, const
 // expand_lm takes it, se / se2 / emax the unweighted statistics of its n points.  The frame's two edge residuals (edges) are
 // expanded exactly as K1's edge tail does and added to the row.
 __device__ __forceinline__ void frame_row_write(const ProblemView& pv, const PoseConsts& pc, int64_t f, int64_t n, const double* S,
-                                                double cost_term, double se, double se2, double emax, bool loss, bool edges,
+                                                double cost_term, double se, double se2, double emax, int loss, bool edges,
                                                 double* row) {
   double plane[4], m[3], c;
 #pragma unroll
@@ -423,7 +456,8 @@ __device__ __forceinline__ void frame_row_write(const ProblemView& pv, const Pos
 // bit-reproducible from run to run, and optionally runs the LM update.
 // LOOP: the instantiation for single-block grids that runs the whole LM loop inside one launch (args.loop_sweeps sweeps at
 // most); kept apart so that the streaming instantiations do not carry the loop's bookkeeping in registers.
-template <bool LOSS, int MODE, bool PLANAR, bool LOOP = false>
+// LOSS: the loss kind (LossKind, clc_expand.cuh).
+template <int LOSS, int MODE, bool PLANAR, bool LOOP = false>
 __global__ void __launch_bounds__(kThreads, kBlocksPerSM)
 clc_sweep_kernel(ProblemView pv, SweepArgs args) {
   constexpr int NOUT = (MODE == kModeClosedForm) ? kMaxOut : kNumSums;
@@ -549,8 +583,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         double m[3], c;
         frame_consts(pc, plane, m, &c);
         const double cnt = (double)(pv.offsets[f + 1] - pv.offsets[f]);
-        double cost_term = row[10];  // loss off: sum e^2
-        if (LOSS) cost_term = log(row[10]) + row[11] * 0.693147180559945309417232121458;
+        double cost_term = row[10];  // other kinds: sum rho~(e)
+        if (LOSS == kLossCauchy) cost_term = log(row[10]) + row[11] * 0.693147180559945309417232121458;
         expand_lm(plane, m, c, 1.0 / cnt, row, LOSS, cost_term, pv.a2, out);
       } else {
         expand_closed_form(plane, row, out);
@@ -581,7 +615,9 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       const double* row = tile + lane * kTileStride;
       const double* rx = ftile + lane * 3;
       const int64_t f = __double_as_longlong(row[12]);
-      const double cost_term = LOSS ? log(row[10]) + row[11] * 0.693147180559945309417232121458 : rx[1];
+      // no loss: the frame's sum e^2 (the sweep does not accumulate it twice); Huber / soft-L1: the summed rho~(e)
+      const double cost_term = LOSS == kLossCauchy ? log(row[10]) + row[11] * 0.693147180559945309417232121458
+                               : LOSS == kLossNone ? rx[1] : row[10];
       frame_row_write(pv, pc, f, pv.offsets[f + 1] - pv.offsets[f], row, cost_term, rx[0], rx[1], rx[2], LOSS,
                       args.use_edges && pv.n_edges > 0, args.frame_rows + f * kRowDoubles);
     }
@@ -644,6 +680,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     }
     Moments a;
     moments_clear<LOSS>(a);
+    // Huber's a (sqrt(a^2) is exact, clc_expand.cuh), once per sweep
+    const double huber_a = LOSS == kLossHuber ? sqrt(pv.a2) : 0.0;
     bool open = false;  // the current piece has accumulated points
     FrameSums fx;       // kModeFrames only
     frame_sums_clear(fx);
@@ -662,14 +700,14 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) em = nan_max(em, __shfl_xor_sync(0xffffffffu, em, o));
       }
-      if (LOSS) {
+      if (LOSS == kLossCauchy) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
           pr *= __shfl_xor_sync(0xffffffffu, pr, o);  // 32 mantissas in [1,2): product < 2^32
           es += __shfl_xor_sync(0xffffffffu, es, o);
         }
       } else {
-        v[10] = pr;  // sum of e^2
+        v[10] = pr;  // sum of e^2 / rho~(e)
       }
       if constexpr (MODE == kModeSegments) {
         // every piece leaves raw -- the moments and the cost (loss: product and exponent): a whole frame to its row of
@@ -681,8 +719,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         double* dst = kind == kPieceWhole
                           ? args.frame_rows + f * kSegRawDoubles
                           : args.frame_slots + (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kSlotDoubles;
-        if (lane < 10 || (!LOSS && lane == 10)) dst[lane] = v[0];
-        if (LOSS && lane == 10) dst[10] = pr;
+        if (lane < 10 || (LOSS != kLossCauchy && lane == 10)) dst[lane] = v[0];
+        if (LOSS == kLossCauchy && lane == 10) dst[10] = pr;
         if (lane == 11) dst[11] = (double)es;
         moments_clear<LOSS>(a);
         open = false;
@@ -694,15 +732,15 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
         // kModeFrames: a piece of a frame that crosses a range end -> this warp's head or tail slot, raw (clc_frames.cuh)
         double* slot = args.frame_slots + (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kSlotDoubles;
         if (lane < 10 || lane == 12 || lane == 13) slot[lane] = v[0];
-        if (lane == 10) slot[10] = LOSS ? pr : 0.0;
+        if (lane == 10) slot[10] = LOSS == kLossCauchy ? pr : LOSS == kLossNone ? 0.0 : v[0];
         if (lane == 11) slot[11] = (double)es;
         if (lane == 14) slot[14] = em;
         if (lane == 15) slot[15] = (double)piece_n;
       } else {
         {
           double* row = tile + n_tile * kTileStride;
-          if (lane < 10 || (!LOSS && lane == 10)) row[lane] = v[0];
-          if (LOSS && lane == 10) row[10] = pr;
+          if (lane < 10 || (LOSS != kLossCauchy && lane == 10)) row[lane] = v[0];
+          if (LOSS == kLossCauchy && lane == 10) row[10] = pr;
           if (lane == 11) row[11] = (double)es;
           if (lane == 12) row[12] = __longlong_as_double(f);
         }
@@ -768,7 +806,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
           // the whole stage belongs to one frame: no masks
 #pragma unroll
           for (int g = 0; g < G; ++g) {
-            process2<LOSS, MODE == kModeLM || MODE == kModeSegments, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2);
+            process2<LOSS, MODE == kModeLM || MODE == kModeSegments, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2,
+                                                                            huber_a, pv.a2);
             if (MODE == kModeFrames) frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], true, true, m0, m1, m2, c);
           }
         } else {
@@ -783,16 +822,16 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
               const double2 Xm = make_double2(v0 ? X[g].x : 0.0, v1 ? X[g].y : 0.0);
               const double2 Ym = make_double2(v0 ? Y[g].x : 0.0, v1 ? Y[g].y : 0.0);
               const double2 Zm = make_double2(v0 ? Z[g].x : 0.0, v1 ? Z[g].y : 0.0);
-              process2<LOSS, true, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, pv.inv_a2);
+              process2<LOSS, true, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, pv.inv_a2, huber_a, pv.a2);
               continue;
             }
             process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2,
-                                            c, pv.inv_a2);
+                                            c, pv.inv_a2, huber_a, pv.a2);
             if (MODE == kModeFrames)
               frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2, c);
           }
         }
-        if (LOSS) renormalise(a);
+        if (LOSS == kLossCauchy) renormalise(a);
         open = true;
         if (MODE == kModeFrames) piece_n += hi - q;
         q = hi;
@@ -835,12 +874,8 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       frame_consts(pc, plane, m, &c);
       const double x = pv.edge_pt[i * 3], y = pv.edge_pt[i * 3 + 1], z = pv.edge_pt[i * 3 + 2];
       const double e = fma(m[0], x, fma(m[1], y, fma(m[2], z, c)));
-      double w = 1.0, cost_term = e * e;
-      if (LOSS) {
-        const double u = fma(e * pv.inv_a2, e, 1.0);
-        w = 1.0 / u;
-        cost_term = log(u);
-      }
+      double w, cost_term;
+      loss_weight(LOSS, e, pv.a2, pv.inv_a2, &w, &cost_term);
       const double S[10] = {w, w * x, w * y, w * z, w * x * x, w * x * y, w * x * z, w * y * y, w * y * z, w * z * z};
       expand_lm(plane, m, c, 1.0 / (double)cnt, S, LOSS, cost_term, pv.a2, out);
     }
@@ -1063,7 +1098,7 @@ __global__ void clc_lm_kernel(LmState* lm, const double* sums) {
 // One thread per frame: an empty frame gets a row of zeros; a split frame (clc_frames.cuh) adds the tail slot of its first warp
 // and the head slots of the following warps, in warp order (the row is bit-reproducible), and expands them into its row; the
 // rows of the other frames were written by the sweep.
-template <bool LOSS>
+template <int LOSS>
 __global__ void clc_frame_fixup_kernel(ProblemView pv, const double* pose7, int edges, const double* __restrict__ slots,
                                        double* __restrict__ rows) {
   const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1084,7 +1119,7 @@ __global__ void clc_frame_fixup_kernel(ProblemView pv, const double* pose7, int 
     const double* s = slots + frame_slot(w, w0);
 #pragma unroll
     for (int k = 0; k < 10; ++k) S[k] += s[k];
-    cost_term += LOSS ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[13];
+    cost_term += LOSS == kLossCauchy ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : LOSS == kLossNone ? s[13] : s[10];
     se += s[12];
     se2 += s[13];
     emax = nan_max(emax, s[14]);

@@ -47,7 +47,7 @@ __global__ void clc_segment_consts_kernel(ProblemView pv, const int32_t* __restr
 // Expands the summed pieces of frame f (S = 10 moments, cost_term as expand_lm takes it) into its row of kNumSums doubles at its
 // segment's pose: m, c of the frame and of its two edge residuals come from `consts` (SweepArgs::seg_consts).
 __device__ __forceinline__ void segment_row_write(const ProblemView& pv, const double* consts, int64_t f, const double* S,
-                                                  double cost_term, bool loss, bool edges, double* row) {
+                                                  double cost_term, int loss, bool edges, double* row) {
   double plane[4], m[3];
 #pragma unroll
   for (int k = 0; k < 4; ++k) plane[k] = pv.plane[f * 4 + k];
@@ -73,7 +73,7 @@ __device__ __forceinline__ void segment_row_write(const ProblemView& pv, const d
 
 // Expansion after a kModeSegments sweep, clc_frame_fixup_kernel's sibling: one thread per frame.  An empty frame gets a row of zeros;
 // a whole frame's raw row (kSegRawDoubles), or a split frame's pieces added in warp order, are expanded at its segment's pose.
-template <bool LOSS>
+template <int LOSS>
 __global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restrict__ consts, int edges, const int* done,
                                          const double* __restrict__ raw, const double* __restrict__ slots,
                                          double* __restrict__ rows) {
@@ -93,7 +93,7 @@ __global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restric
     const double* s = w0 == w1 ? raw + f * kSegRawDoubles : slots + frame_slot(w, w0);
 #pragma unroll
     for (int k = 0; k < 10; ++k) S[k] += s[k];
-    cost_term += LOSS ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[10];
+    cost_term += LOSS == kLossCauchy ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[10];
   }
   segment_row_write(pv, consts, f, S, cost_term, LOSS, edges != 0, row);
 }

@@ -31,7 +31,7 @@ constexpr int64_t kSmallMaxResiduals = (int64_t)kSmallThreads * kSmallCluster * 
 
 // EVAL: one evaluation at `eval_pose` instead of the LM loop -- the 28 sums go to `eval_sums` (clc_eval / clc_information of a
 // small problem: the same residual code, no LM state touched).
-template <bool LOSS, bool EVAL = false>
+template <int LOSS, bool EVAL = false>
 __global__ void __cluster_dims__(kSmallCluster, 1, 1) __launch_bounds__(kSmallThreads, 1)
 clc_small_lm_kernel(ProblemView pv, LmState* lm, int max_sweeps, int use_edges, const double* eval_pose, double* eval_sums) {
   cg::cluster_group cluster = cg::this_cluster();

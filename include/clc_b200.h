@@ -366,6 +366,8 @@ int clc_problem_trim(const clc_problem* src, const double pose7[7], const double
  * problem, so shard boundaries move and kept points may cross devices.  They are read over the peer links under the same
  * temporary memory-pool grants as clc_group_subset's. */
 int clc_group_trim(const clc_group* src, const double pose7[7], const double* max_abs_e, clc_group** out);
+/* clc_problem_set_loss on every shard of g (the clc_group_* calls use it; clc_group_subset / clc_group_trim inherit it). */
+int clc_group_set_loss(clc_group* g, int kind, double a);
 /* The device list the reference-facing drop-in uses (its signatures have no device argument): environment variable
  * CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device only).  Writes at most `cap` ordinals. */
 int clc_default_devices(int* devices, int cap, int* n);
@@ -405,6 +407,28 @@ int clc_problem_streamed_bytes(const clc_problem* p, int64_t* bytes);
  * every warp of the grid a 256-point stage (about 4*10^5 points on an H100) are latency-bound and stay on the general
  * kernels in either mode (environment override for tests: CLC_PLANAR_MIN_POINTS). */
 int clc_problem_set_planar_mode(clc_problem* p, int mode);
+/* Robust losses (Ceres' LossFunction objects).  Every frame scales its residuals r = s e by s = 1/sqrt(#points) and uses the
+ * loss with parameter a*s (reference src/LaseCamCalCeres.cpp:249); the scale cancels from the weights.  With z = e^2/a^2, a
+ * frame's cost is 1/2 s^2 sum rho~(e) over its points and edge residuals:
+ *   CLC_LOSS_NONE      no loss               w = 1                          rho~ = e^2
+ *   CLC_LOSS_CAUCHY    CauchyLoss(a*s)       w = 1/(1+z)                    rho~ = a^2 log(1+z)
+ *   CLC_LOSS_HUBER     HuberLoss(a*s)        w = 1 if |e| <= a, else a/|e|  rho~ = e^2 if |e| <= a, else 2a|e| - a^2
+ *   CLC_LOSS_SOFT_L1   SoftLOneLoss(a*s)     w = 1/sqrt(1+z)                rho~ = 2a^2 (sqrt(1+z) - 1)
+ * A point with |e| == a is a Huber inlier.  The reference hard-codes CauchyLoss(0.05*scale) (:248 keeps a HuberLoss line
+ * commented out); creation maps use_loss = 1 to CAUCHY(cauchy_a) and use_loss = 0 to NONE(cauchy_a). */
+#define CLC_LOSS_NONE 0
+#define CLC_LOSS_CAUCHY 1
+#define CLC_LOSS_HUBER 2
+#define CLC_LOSS_SOFT_L1 3
+/* The loss of every later clc_eval, clc_solve_lm, clc_frame_report, clc_eval_segments, clc_solve_lm_segments and
+ * clc_bench_eval / _frame_report / _segments call on p; clc_problem_subset and clc_problem_trim inherit it.  clc_information,
+ * clc_closed_form and the segment information never use a loss, clc_problem_line_fit keeps its own CauchyLoss(cauchy_a) and
+ * the trim's distances are raw: none of them change.  Fails with CLC_ERR_INVALID, leaving p unchanged, for an unknown kind,
+ * or an a that is not finite and positive with a^2 a normal double.  On a problem attached to a communicator every rank must
+ * set the same loss (not checked). */
+int clc_problem_set_loss(clc_problem* p, int kind, double a);
+/* The loss kind (CLC_LOSS_*) and parameter a of p. */
+int clc_problem_get_loss(const clc_problem* p, int* kind, double* a);
 /* Statistics of this process's most recent host -> HBM point upload: wall time of the pipeline, time the issuing thread
  * waited for the pack threads, bytes that crossed PCIe (16 per point while every z is 0, else 24), chunks, pack threads,
  * direct = 1 when the caller's buffer was pinned and used as the DMA source.  Any pointer may be NULL. */
