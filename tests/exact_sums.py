@@ -8,10 +8,16 @@ the absolute values of what the kernel's algorithm adds and cancels to form that
 
     |got_k - ref_k| <= GAMMA * A_k
 
-for every output.  GAMMA = 1e-13 (about 450 u, u = 2^-53) covers the depth of the kernel's float64 summation: a lane adds at
-most a few hundred points of one warp range, then 5 butterfly levels, one tile flush per 32 pieces, 12 warps per block and
-~10 blocks in each of 13 gather parts followed by the 13 parts -- well under 450 additions on any path, each with a relative
-error of at most u of a partial sum bounded by A_k -- plus a handful of roundings in the per-frame expansion.
+for every output.  GAMMA = 1e-13 (about 450 u, u = 2^-53) covers the depth of the kernel's float64 summation.  Inside a frame a
+lane keeps adding until the frame or its warp range ends: 2 of every 64 points, so up to per_warp / 32 additions -- about 3 950
+at 2*10^8 points, whose warp ranges hold ~126 000 points, when the frames are longer than a warp range.  Then come 5 butterfly
+levels, one tile flush per 32 pieces, 12 warps per block and ~10 blocks in each of 13 gather parts followed by the 13 parts,
+and a handful of roundings in the per-frame expansion: a depth n of about 4 100 on the longest path.  The worst-case bound of
+recursive summation, (n - 1) u sum |x_i|, would allow ~9 GAMMA there; the bound that holds is the probabilistic one of Higham
+and Mary (SIAM J. Sci. Comput. 41 (2019) A2815, Theorem 3.1): with roundings independent and of mean zero, the error is at
+most (exp(lambda sqrt(n) u + n u^2 / (1 - u)) - 1) sum |x_i| ~ lambda sqrt(n) u sum |x_i| with probability at least
+1 - 2 n exp(-lambda^2 (1 - u)^2 / 2).  With n = 4 100 and lambda = 13 that is 9.2e-14 * A_k < GAMMA, failing with probability
+below 1e-32 per output.  tests/test_gpu_at_scale.py runs that depth (100 frames of 2*10^6 points) and measures it.
 
 Magnitudes (s^2 = 1 / #points of the frame, w the Cauchy weight, n the plane normal, m = R^T n, p the point):
   * rounding of the raw distance e = m.p + c, c = n.t + d, is bounded by a few u times L_e = |m||p| + |n||t| + |d|;
