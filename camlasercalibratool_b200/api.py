@@ -218,6 +218,24 @@ def _segments(seg_offsets, poses, n_frames):
     return off, x, W
 
 
+MAX_POSES = 1024
+
+
+def _poses(poses):
+    """K poses [K, 7] for clc_eval_poses / clc_solve_lm_starts -> the float64 array of the C ABI and K (checked before any device
+    work: the library checks them too)."""
+    x = np.asarray(poses)
+    if x.ndim != 2 or x.shape[1] != 7 or not (np.issubdtype(x.dtype, np.floating) or np.issubdtype(x.dtype, np.integer)):
+        raise ValueError(f"poses must be a real array of shape (K, 7), not {x.shape} {x.dtype}")
+    K = x.shape[0]
+    if not 1 <= K <= MAX_POSES:
+        raise ValueError(f"the number of poses must lie in [1, {MAX_POSES}], not {K}")
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    if not np.all(np.isfinite(x)):
+        raise ValueError("poses must be finite")
+    return x, K
+
+
 def default_options(**kw) -> LmOptions:
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
@@ -470,6 +488,32 @@ class Problem:
                   for s in range(W)]
         return x, list(summaries), traces
 
+    # ---- one calibration at many poses (multi-start) ----
+    def eval_poses(self, poses):
+        """eval() at every pose poses[k] of [K, 7], from ONE shared pass over the points (clc_eval_poses).  Returns
+        (cost [K], H [K, 6, 6], g [K, 6]); pose k's bytes depend on poses[k] only."""
+        x, K = _poses(poses)
+        cost, H, g = np.empty(K), np.empty((K, 6, 6)), np.empty((K, 6))
+        _lib.check(self._L.clc_eval_poses(self._h, K, _dp(x), _dp(H), _dp(g), _dp(cost)), "clc_eval_poses")
+        return cost, H, g
+
+    def solve_starts(self, poses, options: LmOptions | None = None, trace_cap=0):
+        """solve() from every start pose poses[k] of [K, 7], the K solves advancing side by side on shared sweeps
+        (clc_solve_lm_starts).  Returns (poses [K, 7], summaries [K] of LmSummary, traces: one list of LmIteration per start,
+        empty without trace_cap, best): best is the start of the lowest final cost that did not fail (lowest index on a tie), -1
+        when every start failed.  summaries[k].device_ms is the time of the whole call."""
+        x, K = _poses(poses)
+        x = x.copy()
+        o = options if options is not None else default_options()
+        summaries = (LmSummary * K)()
+        tr = (LmIteration * (K * trace_cap))() if trace_cap > 0 else None
+        best = C.c_int64()
+        _lib.check(self._L.clc_solve_lm_starts(self._h, K, _dp(x), C.byref(o), summaries, tr, int(trace_cap), C.byref(best)),
+                   "clc_solve_lm_starts")
+        traces = [[tr[k * trace_cap + i] for i in range(min(summaries[k].num_iterations, trace_cap))] if trace_cap > 0 else []
+                  for k in range(K)]
+        return x, list(summaries), traces, best.value
+
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()
         _lib.check(self._L.clc_closed_form(self._h, _dp(T), C.byref(un), _dp(AtA), _dp(Atb)), "clc_closed_form")
@@ -513,6 +557,13 @@ class Problem:
         off, x, W = _segments(seg_offsets, poses, self.sizes()[0])
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_segments(self._h, W, _ip(off), _dp(x), int(n), int(bool(flush_l2)), ms), "clc_bench_segments")
+        return np.array(ms[:], dtype=np.float64)
+
+    def bench_poses(self, poses, n, flush_l2=True):
+        """Device time of n evaluations of eval_poses (without the copy to the host; clc_bench_poses), ms each."""
+        x, K = _poses(poses)
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_poses(self._h, K, _dp(x), int(n), int(bool(flush_l2)), ms), "clc_bench_poses")
         return np.array(ms[:], dtype=np.float64)
 
     def bench_subset(self, keep, n, flush_l2=True):

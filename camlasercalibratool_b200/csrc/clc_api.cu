@@ -350,21 +350,31 @@ int set_device(const clc_problem* p) {
 // kModeFrames: frame_rows / frame_slots receive the per-frame report (clc_frame_fixup_kernel finishes it)
 // the one-cluster kernel of a loss kind (clc::LossKind): one evaluation (EVAL) or the whole LM solve; nullptr for an unknown kind
 using SmallFn = void (*)(clc::ProblemView, clc::LmState*, int, int, const double*, double*);
-template <bool EVAL>
+// POSES: the kernel that runs one cluster per pose in one launch (clc_eval_poses, clc_solve_lm_starts)
+template <bool EVAL, bool POSES = false>
 SmallFn small_fn(int loss) {
   switch (loss) {
-    case clc::kLossNone: return clc::clc_small_lm_kernel<clc::kLossNone, EVAL>;
-    case clc::kLossCauchy: return clc::clc_small_lm_kernel<clc::kLossCauchy, EVAL>;
-    case clc::kLossHuber: return clc::clc_small_lm_kernel<clc::kLossHuber, EVAL>;
-    case clc::kLossSoftL1: return clc::clc_small_lm_kernel<clc::kLossSoftL1, EVAL>;
+    case clc::kLossNone: return POSES ? clc::clc_small_poses_kernel<clc::kLossNone, EVAL> : clc::clc_small_lm_kernel<clc::kLossNone, EVAL>;
+    case clc::kLossCauchy: return POSES ? clc::clc_small_poses_kernel<clc::kLossCauchy, EVAL> : clc::clc_small_lm_kernel<clc::kLossCauchy, EVAL>;
+    case clc::kLossHuber: return POSES ? clc::clc_small_poses_kernel<clc::kLossHuber, EVAL> : clc::clc_small_lm_kernel<clc::kLossHuber, EVAL>;
+    case clc::kLossSoftL1: return POSES ? clc::clc_small_poses_kernel<clc::kLossSoftL1, EVAL> : clc::clc_small_lm_kernel<clc::kLossSoftL1, EVAL>;
     default: return nullptr;
   }
 }
 
+// kModePoses: the tile of running poses a launch walks, and where every pose's constants, rows and slots lie (SweepArgs)
+struct PoseTile {
+  const int* active;
+  const int* count;
+  int tile0;
+  int64_t consts_stride, rows_stride, slots_stride;
+};
+
 // loss: the loss kind of the sweep (clc::LossKind)
 int launch_sweep(clc_problem* p, int mode, int loss, bool edges, const double* d_pose, const int* d_done,
                  clc::LmState* d_lm, bool collective = true, bool pdl = false, int loop_sweeps = 1, bool l2_hints = false,
-                 double* frame_rows = nullptr, double* frame_slots = nullptr, const double* seg_consts = nullptr) {
+                 double* frame_rows = nullptr, double* frame_slots = nullptr, const double* seg_consts = nullptr,
+                 const PoseTile* pose_tile = nullptr) {
   clc::SweepArgs a;
   a.pose7 = d_pose;
   a.done = d_done;
@@ -385,6 +395,12 @@ int launch_sweep(clc_problem* p, int mode, int loss, bool edges, const double* d
   a.frame_rows = frame_rows;
   a.frame_slots = frame_slots;
   a.seg_consts = seg_consts;
+  a.pose_active = pose_tile != nullptr ? pose_tile->active : nullptr;
+  a.pose_count = pose_tile != nullptr ? pose_tile->count : nullptr;
+  a.pose_tile0 = pose_tile != nullptr ? pose_tile->tile0 : 0;
+  a.pose_consts_stride = pose_tile != nullptr ? pose_tile->consts_stride : 0;
+  a.pose_rows_stride = pose_tile != nullptr ? pose_tile->rows_stride : 0;
+  a.pose_slots_stride = pose_tile != nullptr ? pose_tile->slots_stride : 0;
   if (p->nranks > 1 && p->allreduce_mode == 1 && collective) {
     clc_comm* c = p->comm_obj;
     a.nranks = c->nranks;
@@ -420,6 +436,15 @@ int launch_sweep(clc_problem* p, int mode, int loss, bool edges, const double* d
         a.nranks > 1)
       return fail(CLC_ERR_INVALID, "internal: bad segmented sweep");
     const SweepFn fn = sweep_fn<clc::kModeSegments>(loss, p->planar);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+    le = cudaLaunchKernelEx(&cfg, fn, v, a);
+  } else if (mode == clc::kModePoses) {
+    // one calibration at many poses: as the segmented sweep, for the tile of running poses `pose_tile` names
+    if (frame_rows == nullptr || frame_slots == nullptr || seg_consts == nullptr || pose_tile == nullptr || d_lm != nullptr ||
+        loop_sweeps > 1 || a.nranks > 1)
+      return fail(CLC_ERR_INVALID, "internal: bad multi-pose sweep");
+    const SweepFn fn = sweep_fn<clc::kModePoses>(loss, p->planar);
     if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
@@ -1823,6 +1848,278 @@ int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg
   return CLC_OK;
 }
 
+// ---- one calibration at many poses (multi-start) -------------------------------------------------------------------
+// Problems the one-cluster kernel serves run one cluster per pose in one launch (clc_small.cuh, POSES); every other problem runs
+// the segmented iteration over a pose-major virtual segmentation (clc_segments.cuh) with the multi-pose sweep kModePoses, which
+// reads every stage once for a tile of up to kPoseTile running poses.
+
+namespace {
+
+constexpr int64_t kMaxPoses = 1024;
+
+// rejects bad arguments before the device is touched
+int check_poses(const clc_problem* p, int64_t K, const double* poses) {
+  if (!p || !poses) return fail(CLC_ERR_INVALID, "NULL argument");
+  if (K < 1 || K > kMaxPoses) return fail(CLC_ERR_INVALID, "n_poses outside [1, 1024]");
+  for (int64_t i = 0; i < 7 * K; ++i)
+    if (!clc::is_finite(poses[i])) return fail(CLC_ERR_INVALID, "a pose entry is not finite");
+  if (p->comm_obj != nullptr || p->nranks > 1) return fail(CLC_ERR_STATE, "multi-pose calls run on a problem without a communicator");
+  return CLC_OK;
+}
+
+// The device buffers of one multi-pose call on K1: SegmentRun over the K * n_frames virtual rows, plus the running poses.
+struct PoseRun {
+  SegmentRun s;
+  int64_t K = 0;
+  int* active = nullptr;  // [K] running poses, then [3]: poses still running, all done, number of listed poses
+  int* running() const { return active + K; }
+  int* count() const { return active + K + 2; }
+  ~PoseRun() {
+    if (s.p && active) {
+      cudaSetDevice(s.p->device);
+      cudaFreeAsync(active, s.p->stream);
+    }
+  }
+};
+
+// the plan, the work buffers and the full list of running poses 0 .. K-1 on the device
+int poses_prepare(clc_problem* p, int64_t K, PoseRun* r) {
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  const int64_t N = p->n_frames;
+  r->s.p = p;
+  r->s.W = K;
+  r->K = K;
+  const std::vector<int64_t> off = clc::pose_segment_offsets(N, K);
+  const clc::SegmentPlan plan = clc::segment_plan(N * K, K, off.data());
+  r->s.n_chunks = (int64_t)plan.chunk_offsets.size() - 1;
+  const size_t rows = (size_t)(N * K);
+  if ((rc = seg_alloc(p, &r->s.chunk_offsets, plan.chunk_offsets.size())) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.seg_chunks, plan.seg_chunks.size())) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.consts, (size_t)K * (size_t)(N + p->n_edges) * 4)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.raw, rows * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->s.rows, rows * clc::kNumSums)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.slots, (size_t)K * p->grid * clc::kWarps * 2 * clc::kSlotDoubles)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.partials, (size_t)r->s.n_chunks * clc::kNumSums)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->active, (size_t)K + 3)) != CLC_OK)
+    return rc;
+  CLC_CUDA(cudaMemcpyAsync(r->s.chunk_offsets, plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
+                           cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->s.seg_chunks, plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(), cudaMemcpyHostToDevice,
+                           p->stream));
+  std::vector<int> active((size_t)K + 3);
+  for (int64_t k = 0; k < K; ++k) active[(size_t)k] = (int)k;
+  active[(size_t)K] = (int)K;  // running
+  active[(size_t)K + 1] = 0;   // done
+  active[(size_t)K + 2] = (int)K;  // listed
+  // pageable sources: each copy has read its source when it returns
+  CLC_CUDA(cudaMemcpyAsync(r->active, active.data(), sizeof(int) * active.size(), cudaMemcpyHostToDevice, p->stream));
+  return CLC_OK;
+}
+
+// One shared iteration of the running poses: pose k at poses[k * pose_stride] on the device.  sums: [K * kNumSums] or nullptr;
+// cores: the solve's LmCores -- lm_update runs on every running pose, and the list of running poses is compacted afterwards.
+int poses_iteration(const PoseRun& r, int loss, bool edges, const double* poses, int64_t pose_stride, double* sums,
+                    clc::LmCore* cores, clc_lm_iteration* trace, int trace_cap) {
+  clc_problem* p = r.s.p;
+  const int64_t K = r.K, N = p->n_frames;
+  int* done = cores != nullptr ? r.running() + 1 : nullptr;
+  const bool with_edges = edges && p->n_edges > 0;
+  const clc::ProblemView v = make_view(p);
+  const int threads = 256;
+  const int64_t consts_stride = (N + p->n_edges) * 4;
+  const int64_t raw_stride = N * clc::kSegRawDoubles;
+  const int64_t slots_stride = (int64_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles;
+  if (N > 0) {
+    const dim3 fb((unsigned)((N + threads - 1) / threads), (unsigned)K);
+    clc::clc_pose_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.active, r.count(), poses, pose_stride, with_edges ? 1 : 0,
+                                                               r.s.consts, consts_stride);
+    CLC_LAUNCH_CHECK();
+    for (int64_t t0 = 0; t0 < K; t0 += clc::kPoseTile) {
+      const PoseTile tile{r.active, r.count(), (int)t0, consts_stride, raw_stride, slots_stride};
+      int rc = launch_sweep(p, clc::kModePoses, loss, with_edges, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
+                            /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw, r.s.slots, r.s.consts, &tile);
+      if (rc != CLC_OK) return rc;
+    }
+    void (*fixup)(clc::ProblemView, const int*, const int*, const double*, int64_t, int, const double*, int64_t, const double*,
+                  int64_t, double*) =
+        loss == clc::kLossCauchy  ? clc::clc_pose_fixup_kernel<clc::kLossCauchy>
+        : loss == clc::kLossHuber ? clc::clc_pose_fixup_kernel<clc::kLossHuber>
+        : loss == clc::kLossSoftL1 ? clc::clc_pose_fixup_kernel<clc::kLossSoftL1>
+                                   : clc::clc_pose_fixup_kernel<clc::kLossNone>;
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.active, r.count(), r.s.consts, consts_stride, with_edges ? 1 : 0, r.s.raw, raw_stride,
+                                         r.s.slots, slots_stride, r.s.rows);
+    CLC_LAUNCH_CHECK();
+  }
+  if (r.s.n_chunks > 0) {
+    const unsigned cb = (unsigned)((r.s.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+    clc::clc_segment_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.rows, r.s.chunk_offsets, r.s.n_chunks, done,
+                                                                                     r.s.partials);
+    CLC_LAUNCH_CHECK();
+  }
+  const unsigned sb = (unsigned)((K + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+  clc::clc_segment_lm_kernel<<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.partials, r.s.seg_chunks, K, sums, cores, trace,
+                                                                                trace_cap, cores != nullptr ? r.running() : nullptr,
+                                                                                done);
+  CLC_LAUNCH_CHECK();
+  if (cores != nullptr) {
+    clc::clc_pose_compact_kernel<<<1, clc::kPoseCompactThreads, 0, p->stream>>>(cores, (int)K, r.active, r.count());
+    CLC_LAUNCH_CHECK();
+  }
+  return CLC_OK;
+}
+
+// the K2 (one cluster per pose) instantiation of a loss kind, or nullptr
+SmallFn small_poses_fn(int loss, bool eval) { return eval ? small_fn<true, true>(loss) : small_fn<false, true>(loss); }
+
+// The sums of every pose into sums[K * kNumSums] on the device (d_poses: [K * 7] on the device); r is prepared on K1 problems.
+int eval_poses_enqueue(clc_problem* p, int64_t K, const double* d_poses, double* d_sums, const PoseRun* r) {
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
+  if (small_kernel_serves(p, edges)) {
+    const SmallFn fn = small_poses_fn(loss, true);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), nullptr, 1, edges ? 1 : 0, d_poses,
+                                                                                  d_sums);
+    CLC_LAUNCH_CHECK();
+    return CLC_OK;
+  }
+  return poses_iteration(*r, loss, edges, d_poses, 7, d_sums, nullptr, nullptr, 0);
+}
+
+// the work buffers of clc_eval_poses / clc_bench_poses: the poses and sums on the device, and r on K1 problems
+int eval_poses_prepare(clc_problem* p, int64_t K, const double* poses, PoseRun* r) {
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  r->s.p = p;
+  if (!small_kernel_serves(p, p->n_edges > 0) && (rc = poses_prepare(p, K, r)) != CLC_OK) return rc;
+  if ((rc = seg_alloc(p, &r->s.poses, (size_t)K * 7)) != CLC_OK || (rc = seg_alloc(p, &r->s.sums, (size_t)K * clc::kNumSums)) != CLC_OK)
+    return rc;
+  CLC_CUDA(cudaMemcpyAsync(r->s.poses, poses, sizeof(double) * 7 * (size_t)K, cudaMemcpyHostToDevice, p->stream));
+  return CLC_OK;
+}
+
+}  // namespace
+
+int clc_eval_poses(clc_problem* p, int64_t n_poses, const double* poses, double* H36, double* g6, double* cost) {
+  if (!cost) return fail(CLC_ERR_INVALID, "NULL argument");
+  int rc = check_poses(p, n_poses, poses);
+  if (rc != CLC_OK) return rc;
+  PoseRun r;
+  if ((rc = eval_poses_prepare(p, n_poses, poses, &r)) != CLC_OK) return rc;
+  if ((rc = eval_poses_enqueue(p, n_poses, r.s.poses, r.s.sums, &r)) != CLC_OK) return rc;
+  std::vector<double> sums((size_t)n_poses * clc::kNumSums);
+  CLC_CUDA(cudaMemcpyAsync(sums.data(), r.s.sums, sizeof(double) * sums.size(), cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  for (int64_t k = 0; k < n_poses; ++k)
+    eval_post(sums.data() + k * clc::kNumSums, H36 ? H36 + 36 * k : nullptr, g6 ? g6 + 6 * k : nullptr, cost + k);
+  return CLC_OK;
+}
+
+int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const clc_lm_options* opt_in, clc_lm_summary* summaries,
+                        clc_lm_iteration* trace, int trace_cap, int64_t* best) {
+  if (!summaries || trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
+    return fail(CLC_ERR_INVALID, "NULL summaries, or trace_cap outside [0, 256] without a trace array");
+  int rc = check_poses(p, n_poses, poses);
+  if (rc != CLC_OK) return rc;
+  clc_lm_options opt;
+  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
+  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
+  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  if ((rc = set_device(p)) != CLC_OK) return rc;
+  const int64_t K = n_poses;
+  const int loss = p->loss_kind;
+  const bool edges = p->n_edges > 0;
+  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
+  const int max_sweeps = opt.max_num_iterations + 2;
+  std::vector<clc::LmCore> cores((size_t)K);
+  std::vector<clc_lm_iteration> rows;  // [K * trace_cap]
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  if (p->loop_in_kernel >= 1 && fused_lm_update(p) && small_kernel_serves(p, edges)) {
+    // the whole solve of every start in one launch, one cluster per start (the path clc_solve_lm takes for this problem)
+    const SmallFn fn = small_poses_fn(loss, false);
+    if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
+    std::vector<clc::LmState> states((size_t)K);
+    for (int64_t k = 0; k < K; ++k) clc::lm_init(&states[(size_t)k].core, poses + 7 * k, opt);
+    clc::LmState* d_states = nullptr;
+    if ((rc = seg_alloc(p, &d_states, (size_t)K)) != CLC_OK) return rc;
+    struct Free {
+      clc_problem* p;
+      void* b;
+      ~Free() { cudaFreeAsync(b, p->stream); }
+    } free_states{p, d_states};
+    // without a trace only the LmCore at the head of every state travels (the kernel writes the trace rows on the device)
+    const size_t moved = trace_cap > 0 ? sizeof(clc::LmState) : sizeof(clc::LmCore);
+    CLC_CUDA(cudaMemcpy2DAsync(d_states, sizeof(clc::LmState), states.data(), sizeof(clc::LmState), moved, (size_t)K,
+                               cudaMemcpyHostToDevice, p->stream));
+    CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), d_states, max_sweeps, edges ? 1 : 0,
+                                                                                  nullptr, nullptr);
+    CLC_LAUNCH_CHECK();
+    CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+    CLC_CUDA(cudaMemcpy2DAsync(states.data(), sizeof(clc::LmState), d_states, sizeof(clc::LmState), moved, (size_t)K,
+                               cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
+    rows.resize((size_t)K * trace_cap);
+    for (int64_t k = 0; k < K; ++k) {
+      cores[(size_t)k] = states[(size_t)k].core;
+      const int n = std::min(std::min(cores[(size_t)k].n_trace, clc::kTraceMax), trace_cap);
+      for (int i = 0; i < n; ++i) rows[(size_t)k * trace_cap + i] = states[(size_t)k].trace[i];
+    }
+  } else {
+    PoseRun r;
+    if ((rc = poses_prepare(p, K, &r)) != CLC_OK || (rc = seg_alloc(p, &r.s.cores, (size_t)K)) != CLC_OK) return rc;
+    if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, (size_t)K * trace_cap)) != CLC_OK) return rc;
+    for (int64_t k = 0; k < K; ++k) clc::lm_init(&cores[(size_t)k], poses + 7 * k, opt);
+    CLC_CUDA(cudaMemcpyAsync(r.s.cores, cores.data(), sizeof(clc::LmCore) * (size_t)K, cudaMemcpyHostToDevice, p->stream));
+    CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+    // the candidate pose of start k: cores[k].cand, sizeof(LmCore) / 8 doubles apart
+    const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.s.cores) + offsetof(clc::LmCore, cand));
+    const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
+    int launched = 0;
+    while (launched < max_sweeps) {
+      // the first batch is twice as long, as in solve_all
+      const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
+      for (int i = 0; i < batch; ++i)
+        if ((rc = poses_iteration(r, loss, edges, cand, stride, nullptr, r.s.cores, r.s.trace, trace_cap)) != CLC_OK) return rc;
+      launched += batch;
+      CLC_CUDA(cudaMemcpyAsync(p->h_done, r.running(), sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+      CLC_CUDA(sync_stream_low_latency(p->stream));
+      if (*p->h_done == 0) break;  // no start is running
+    }
+    CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+    CLC_CUDA(cudaMemcpyAsync(cores.data(), r.s.cores, sizeof(clc::LmCore) * (size_t)K, cudaMemcpyDeviceToHost, p->stream));
+    rows.resize((size_t)K * trace_cap);
+    if (trace_cap > 0)
+      CLC_CUDA(cudaMemcpyAsync(rows.data(), r.s.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
+  }
+  float ms = 0.f;
+  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
+  std::vector<int> term((size_t)K);
+  std::vector<double> final_cost((size_t)K);
+  for (int64_t k = 0; k < K; ++k) {
+    const clc::LmCore& c = cores[(size_t)k];
+    for (int i = 0; i < 7; ++i) poses[7 * k + i] = c.x[i];  // the last accepted point, as clc_solve_lm
+    clc_lm_summary& sm = summaries[k];
+    sm.termination = c.done ? c.done : CLC_TERM_NO_CONVERGENCE;
+    sm.num_iterations = c.n_trace;
+    sm.num_successful_steps = c.num_successful;
+    sm.num_unsuccessful_steps = c.num_unsuccessful;
+    sm.num_sweeps = c.sweeps;
+    sm.reserved = 0;
+    sm.initial_cost = c.initial_cost;
+    sm.final_cost = c.x_cost;
+    sm.device_ms = ms;
+    term[(size_t)k] = sm.termination;
+    final_cost[(size_t)k] = sm.final_cost;
+    const int n = std::min(c.n_trace, trace_cap);
+    for (int i = 0; i < n; ++i) trace[k * trace_cap + i] = rows[(size_t)k * trace_cap + i];
+  }
+  if (best) *best = clc::best_start(K, term.data(), final_cost.data(), CLC_TERM_FAILURE);
+  return CLC_OK;
+}
+
 // ---- LineFittingCeres, batched ------------------------------------------------------------------------------------
 
 int clc_problem_line_fit(clc_problem* p, double* lines, int max_num_iterations, double* info) {
@@ -3149,6 +3446,18 @@ int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_of
   return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
     return segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
   });
+}
+
+int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n, int flush_l2, float* ms_each) {
+  if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_poses(p, n_poses, poses);
+  if (rc != CLC_OK) return rc;
+  PoseRun r;
+  if ((rc = eval_poses_prepare(p, n_poses, poses, &r)) != CLC_OK) return rc;
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return eval_poses_enqueue(p, n_poses, r.s.poses, r.s.sums, &r); });
 }
 
 int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each) {

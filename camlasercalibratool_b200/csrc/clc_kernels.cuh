@@ -82,7 +82,13 @@ __host__ __device__ constexpr int frames_smem_bytes(bool planar) {
 // A raw row: 10 moments, the cost (Cauchy: product of (1 + e^2/a^2) with its exponent taken out; other kinds: sum rho~(e),
 // clc_expand.cuh) and that exponent -- the layout of the first 12 doubles of a split-frame slot.
 constexpr int kSegRawDoubles = 12;
-enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3 };
+// kModePoses: one calibration at many poses (clc_eval_poses, clc_solve_lm_starts) -- every stage is read once and walked once per
+// pose of a tile of at most kPoseTile poses, with that pose's frame constants; every piece leaves raw as in kModeSegments, to
+// that pose's rows and slots.  A piece that continues past a stage waits in a per-warp, per-pose accumulator that takes the
+// place of the tile (12 doubles per pose: 10 moments, cost, exponent).
+constexpr int kPoseTile = 32;
+static_assert(kPoseTile * kSegRawDoubles <= kTileDoublesPerWarp, "the open pieces of a pose tile live in the warp's tile");
+enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3, kModePoses = 4 };
 
 // Device-resident problem (read-only for the sweeps).
 struct ProblemView {
@@ -135,6 +141,15 @@ struct SweepArgs {
   double* frame_slots;  // [total warps * 2 * kSlotDoubles] head / tail pieces of split frames (clc_frames.cuh)
   // kModeSegments only (frame_rows then holds [n_frames * kSegRawDoubles] raw rows; frame_slots as above)
   const double* seg_consts;  // [(n_frames + n_edges) * 4] m, c of every frame, then of every edge residual, at its segment's pose
+  // kModePoses only: pose k's constants at seg_consts + k * pose_consts_stride, its raw rows at frame_rows + k * pose_rows_stride,
+  // its slots at frame_slots + k * pose_slots_stride; this launch walks the poses pose_active[pose_tile0 ..
+  // min(pose_tile0 + kPoseTile, *pose_count))
+  const int* pose_active;
+  const int* pose_count;
+  int pose_tile0;
+  int64_t pose_consts_stride;
+  int64_t pose_rows_stride;
+  int64_t pose_slots_stride;
 };
 
 // ---- small device helpers ---------------------------------------------------------------------------------
@@ -543,7 +558,12 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncwarp();
-  for (int g = 0; g < NST && g < total_chunks; ++g) issue_one(false);
+  // kModePoses: a tile with no running pose reads no point (the list of running poses is final before the launch: no PDL)
+  int first_issue = total_chunks;
+  if constexpr (MODE == kModePoses) {
+    if (*args.pose_count <= args.pose_tile0) first_issue = 0;
+  }
+  for (int g = 0; g < NST && g < first_issue; ++g) issue_one(false);
   __syncwarp();
 
   // Programmatic dependent launch: everything above touched only constant data (the points), so it overlaps the
@@ -553,6 +573,119 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
   if (args.done != nullptr && (*args.done != 0 || (args.error != nullptr && *args.error != 0))) {
     // the LM finished (or an earlier sweep of this solve lost a peer): nothing to do, but the bulk copies already in flight must land before the block may exit
     drain(0);
+    return;
+  }
+
+  if constexpr (MODE == kModePoses) {
+    const int t1 = min(*args.pose_count, args.pose_tile0 + kPoseTile);
+    const int nt = t1 - args.pose_tile0;
+    if (nt <= 0 || n_chunks == 0) {  // no pose of this tile is running (or no points in this range)
+      drain(0);
+      return;
+    }
+    // the open piece of every pose of the tile: lane L < 12 keeps value L of it
+    double* open = tile;
+    for (int j = 0; j < nt; ++j)
+      if (lane < kSegRawDoubles) open[j * kSegRawDoubles + lane] = (LOSS == kLossCauchy && lane == 10) ? 1.0 : 0.0;
+    __syncwarp();
+    const double huber_a = LOSS == kLossHuber ? sqrt(pv.a2) : 0.0;
+    // adds this lane's share of one piece of pose j to its open piece: the lanes' moments are summed across the warp (and the
+    // Cauchy products multiplied), so the sum of a piece does not depend on how many poses share the stage
+    auto fold = [&](const Moments& a, int j) {
+      double v[16] = {a.S0, a.Sx, a.Sy, a.Sz, a.Sxx, a.Sxy, a.Sxz, a.Syy, a.Syz, a.Szz, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+      double pr = a.prod;
+      int es = a.esum;
+      if (LOSS == kLossCauchy) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          pr *= __shfl_xor_sync(0xffffffffu, pr, o);  // 32 mantissas in [1,2): product < 2^32
+          es += __shfl_xor_sync(0xffffffffu, es, o);
+        }
+      } else {
+        v[10] = pr;
+      }
+      warp_transpose_sum_regs<16>(v, lane);
+      double* o = open + j * kSegRawDoubles;
+      if (lane < 10 || (LOSS != kLossCauchy && lane == 10)) o[lane] += v[0];
+      if (LOSS == kLossCauchy && lane == 10) {
+        Moments m;
+        m.prod = o[10] * pr;  // [1,2) x [1, 2^32): exact exponent bookkeeping as renormalise does
+        m.esum = (int)o[11] + es;
+        renormalise(m);
+        o[10] = m.prod;
+        o[11] = (double)m.esum;
+      }
+    };
+    // the open piece of frame f of pose k leaves raw, as kModeSegments' pieces do, and the accumulator starts afresh
+    auto emit = [&](int j, int k, int64_t f, int64_t f_end) {
+      const int kind = frame_piece_kind(pv.offsets[f], f_end, p0, p1);
+      double* dst = kind == kPieceWhole ? args.frame_rows + k * args.pose_rows_stride + f * kSegRawDoubles
+                                        : args.frame_slots + k * args.pose_slots_stride +
+                                              (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kSlotDoubles;
+      double* o = open + j * kSegRawDoubles;
+      __syncwarp();  // lane 10 of fold wrote the exponent that lane 11 reads here
+      if (lane < kSegRawDoubles) {
+        dst[lane] = o[lane];
+        o[lane] = (LOSS == kLossCauchy && lane == 10) ? 1.0 : 0.0;
+      }
+      __syncwarp();
+    };
+    int64_t f = pv.warp_first_frame[gwarp];
+    int64_t f_end = pv.offsets[f + 1];
+    for (int ch = 0; ch < n_chunks; ++ch) {
+      const int st = ch % NST;
+      const int64_t cb = p0 + (int64_t)ch * CH;
+      const int64_t ce = (cb + CH < p1) ? cb + CH : p1;
+      mbar_wait(bars + st, (uint32_t)(ch / NST) & 1u);
+      const double* sx = ring + st * SST;
+      double2 X[G], Y[G], Z[G];
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+        X[g] = *reinterpret_cast<const double2*>(sx + 64 * g + 2 * lane);
+        Y[g] = *reinterpret_cast<const double2*>(sx + CH + 64 * g + 2 * lane);
+        Z[g] = PLANAR ? make_double2(0.0, 0.0) : *reinterpret_cast<const double2*>(sx + 2 * CH + 64 * g + 2 * lane);
+      }
+      const int64_t f_stage = f, f_end_stage = f_end;
+      for (int j = 0; j < nt; ++j) {
+        const int k = args.pose_active[args.pose_tile0 + j];
+        const double* kc = args.seg_consts + k * args.pose_consts_stride;
+        f = f_stage;
+        f_end = f_end_stage;
+        int64_t q = cb;
+        while (q < ce) {
+          while (f_end <= q) f_end = pv.offsets[++f + 1];  // next non-empty frame
+          const double m0 = kc[f * 4], m1 = kc[f * 4 + 1], m2 = kc[f * 4 + 2], c = kc[f * 4 + 3];
+          const int64_t hi = f_end < ce ? f_end : ce;
+          Moments a;
+          moments_clear<LOSS>(a);
+          if (q == cb && hi == cb + CH) {
+#pragma unroll
+            for (int g = 0; g < G; ++g)
+              process2<LOSS, true, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2, huber_a, pv.a2);
+          } else {
+#pragma unroll
+            for (int g = 0; g < G; ++g) {
+              // as kModeSegments: the points outside the piece are replaced before any arithmetic
+              const int64_t i0 = cb + 64 * g + 2 * lane;
+              const bool v0 = i0 >= q && i0 < hi, v1 = i0 + 1 >= q && i0 + 1 < hi;
+              const double2 Xm = make_double2(v0 ? X[g].x : 0.0, v1 ? X[g].y : 0.0);
+              const double2 Ym = make_double2(v0 ? Y[g].x : 0.0, v1 ? Y[g].y : 0.0);
+              const double2 Zm = make_double2(v0 ? Z[g].x : 0.0, v1 ? Z[g].y : 0.0);
+              process2<LOSS, true, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, pv.inv_a2, huber_a, pv.a2);
+            }
+          }
+          if (LOSS == kLossCauchy) renormalise(a);
+          fold(a, j);
+          q = hi;
+          if (hi == f_end) emit(j, k, f, f_end);
+        }
+      }
+      __syncwarp();
+      if (issued < total_chunks) issue_one(true);
+    }
+    // the last frame continues in the next warp's range: its piece leaves as this warp's tail (or head) slot
+    if (f_end > p1)
+      for (int j = 0; j < nt; ++j) emit(j, args.pose_active[args.pose_tile0 + j], f, f_end);
     return;
   }
 

@@ -57,4 +57,24 @@ inline SegmentPlan segment_plan(int64_t n_frames, int64_t W, const int64_t* seg_
   return p;
 }
 
+// One calibration at K poses (clc_eval_poses, clc_solve_lm_starts): pose k owns all n_frames frames, so its rows form segment k
+// of a pose-major virtual segmentation of K * n_frames rows, seg_offsets[k] = k * n_frames, which segment_plan reduces.
+inline std::vector<int64_t> pose_segment_offsets(int64_t n_frames, int64_t K) {
+  std::vector<int64_t> off((size_t)K + 1);
+  for (int64_t k = 0; k <= K; ++k) off[(size_t)k] = k * n_frames;
+  return off;
+}
+
+// The best of K solves: the lowest final cost among those whose termination is not `failure` (a NaN cost loses to any other),
+// the lowest index on a tie; -1 when every solve failed.
+CLC_HD int64_t best_start(int64_t K, const int* termination, const double* final_cost, int failure) {
+  int64_t best = -1;
+  for (int64_t k = 0; k < K; ++k) {
+    if (termination[k] == failure) continue;
+    const double c = final_cost[k];
+    if (best < 0 || c < final_cost[best] || (final_cost[best] != final_cost[best] && c == c)) best = k;
+  }
+  return best;
+}
+
 }  // namespace clc

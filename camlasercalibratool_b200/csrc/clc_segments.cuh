@@ -10,6 +10,7 @@
 //   4. clc_segment_chunk_kernel    level 1 of the fixed reduction plan (clc_segment_plan.h): the rows of every chunk;
 //   5. clc_segment_lm_kernel       level 2: the chunk partials of every segment, then lm_update on the segment's own LmCore.
 // Every kernel of the iteration is a no-op once every segment has terminated (`done`, raised by the last one).
+// The kernels at the end of the file run the same iteration for one calibration at many poses.
 #pragma once
 
 #include "clc_kernels.cuh"
@@ -17,16 +18,13 @@
 
 namespace clc {
 
-// One thread per frame: the frame constants at the pose of its segment, pose s at poses[s * pose_stride] (the caller's poses, or
-// the candidate of segment s's LmCore); edges: also those of its two edge residuals, behind the frames' (SweepArgs::seg_consts).
-__global__ void clc_segment_consts_kernel(ProblemView pv, const int32_t* __restrict__ frame_seg, const double* poses,
-                                          int64_t pose_stride, int edges, const int* done, double* __restrict__ consts) {
-  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= pv.n_frames || (done != nullptr && *done != 0)) return;
+// The frame constants of frame f at `pose`: m, c of the frame (and, with edges, of its two edge residuals, behind the frames':
+// SweepArgs::seg_consts).
+__device__ __forceinline__ void frame_consts_at(const ProblemView& pv, const double* pose_src, int64_t f, int edges,
+                                                double* __restrict__ consts) {
   double pose[7];
-  const double* src = poses + (int64_t)frame_seg[f] * pose_stride;
 #pragma unroll
-  for (int k = 0; k < 7; ++k) pose[k] = src[k];
+  for (int k = 0; k < 7; ++k) pose[k] = pose_src[k];
   PoseConsts pc;
   make_pose_consts(pose, &pc);
   double plane[4], m[3], c;
@@ -42,6 +40,15 @@ __global__ void clc_segment_consts_kernel(ProblemView pv, const int32_t* __restr
       o[0] = m[0]; o[1] = m[1]; o[2] = m[2]; o[3] = c;
     }
   }
+}
+
+// One thread per frame: the frame constants at the pose of its segment, pose s at poses[s * pose_stride] (the caller's poses, or
+// the candidate of segment s's LmCore).
+__global__ void clc_segment_consts_kernel(ProblemView pv, const int32_t* __restrict__ frame_seg, const double* poses,
+                                          int64_t pose_stride, int edges, const int* done, double* __restrict__ consts) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= pv.n_frames || (done != nullptr && *done != 0)) return;
+  frame_consts_at(pv, poses + (int64_t)frame_seg[f] * pose_stride, f, edges, consts);
 }
 
 // Expands the summed pieces of frame f (S = 10 moments, cost_term as expand_lm takes it) into its row of kNumSums doubles at its
@@ -71,14 +78,13 @@ __device__ __forceinline__ void segment_row_write(const ProblemView& pv, const d
   for (int k = 0; k < kNumSums; ++k) row[k] = out[k];
 }
 
-// Expansion after a kModeSegments sweep, clc_frame_fixup_kernel's sibling: one thread per frame.  An empty frame gets a row of zeros;
-// a whole frame's raw row (kSegRawDoubles), or a split frame's pieces added in warp order, are expanded at its segment's pose.
+// Expansion of frame f after a kModeSegments or kModePoses sweep, clc_frame_fixup_kernel's sibling.  An empty frame gets a row of
+// zeros; a whole frame's raw row (kSegRawDoubles), or a split frame's pieces added in warp order, are expanded at the pose of
+// `consts`.
 template <int LOSS>
-__global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restrict__ consts, int edges, const int* done,
-                                         const double* __restrict__ raw, const double* __restrict__ slots,
-                                         double* __restrict__ rows) {
-  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= pv.n_frames || (done != nullptr && *done != 0)) return;
+__device__ __forceinline__ void segment_fixup_frame(const ProblemView& pv, const double* __restrict__ consts, int edges, int64_t f,
+                                                    const double* __restrict__ raw, const double* __restrict__ slots,
+                                                    double* __restrict__ rows) {
   const int64_t fs = pv.offsets[f], fe = pv.offsets[f + 1];
   double* row = rows + f * kNumSums;
   if (fe <= fs) {
@@ -96,6 +102,16 @@ __global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restric
     cost_term += LOSS == kLossCauchy ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[10];
   }
   segment_row_write(pv, consts, f, S, cost_term, LOSS, edges != 0, row);
+}
+
+// One thread per frame, at its segment's pose.
+template <int LOSS>
+__global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restrict__ consts, int edges, const int* done,
+                                         const double* __restrict__ raw, const double* __restrict__ slots,
+                                         double* __restrict__ rows) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= pv.n_frames || (done != nullptr && *done != 0)) return;
+  segment_fixup_frame<LOSS>(pv, consts, edges, f, raw, slots, rows);
 }
 
 // Level 1: one warp per chunk, lane k < kNumSums adds output k of the chunk's rows in frame order.
@@ -142,6 +158,50 @@ clc_segment_lm_kernel(const double* __restrict__ partials, const int64_t* __rest
   }
   __syncwarp();
   for (int k = lane; k < kLmCoreWords; k += 32) g_core[k] = s_core[warp][k];
+}
+
+
+// ---- one calibration at many poses (clc_eval_poses, clc_solve_lm_starts) ----------------------------------------------------
+// Pose k owns every frame, so the K poses form a pose-major virtual segmentation of K * n_frames rows (segment k = rows
+// [k n_frames, (k + 1) n_frames)) that the chunk and LM kernels above reduce and update unchanged.  Only the running poses are
+// evaluated: pose_active[0 .. *pose_count) lists them (clc_pose_compact_kernel), and blockIdx.y walks that list.
+
+// One thread per frame and running pose: pose k's frame constants at poses[k * pose_stride], to consts + k * consts_stride.
+__global__ void clc_pose_consts_kernel(ProblemView pv, const int* __restrict__ pose_active, const int* pose_count, const double* poses,
+                                       int64_t pose_stride, int edges, double* __restrict__ consts, int64_t consts_stride) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= pv.n_frames || (int)blockIdx.y >= *pose_count) return;
+  const int64_t k = pose_active[blockIdx.y];
+  frame_consts_at(pv, poses + k * pose_stride, f, edges, consts + k * consts_stride);
+}
+
+// One thread per frame and running pose: the rows of pose k after a kModePoses sweep (strides as SweepArgs' pose_*_stride).
+template <int LOSS>
+__global__ void clc_pose_fixup_kernel(ProblemView pv, const int* __restrict__ pose_active, const int* pose_count,
+                                      const double* __restrict__ consts, int64_t consts_stride, int edges,
+                                      const double* __restrict__ raw, int64_t raw_stride, const double* __restrict__ slots,
+                                      int64_t slots_stride, double* __restrict__ rows) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= pv.n_frames || (int)blockIdx.y >= *pose_count) return;
+  const int64_t k = pose_active[blockIdx.y];
+  segment_fixup_frame<LOSS>(pv, consts + k * consts_stride, edges, f, raw + k * raw_stride, slots + k * slots_stride,
+                            rows + k * pv.n_frames * kNumSums);
+}
+
+// One block of kPoseCompactThreads: the poses whose LmCore is still running, in increasing order, to pose_active[0 .. *pose_count).
+constexpr int kPoseCompactThreads = 1024;
+__global__ void __launch_bounds__(kPoseCompactThreads)
+clc_pose_compact_kernel(const LmCore* __restrict__ cores, int n_poses, int* __restrict__ pose_active, int* pose_count) {
+  __shared__ int s_warp[kPoseCompactThreads / 32];
+  const int k = threadIdx.x, lane = k & 31, warp = k >> 5;
+  const bool running = k < n_poses && cores[k].done == 0;
+  const unsigned ballot = __ballot_sync(0xffffffffu, running);
+  if (lane == 0) s_warp[warp] = __popc(ballot);
+  __syncthreads();
+  int base = 0;
+  for (int w = 0; w < warp; ++w) base += s_warp[w];
+  if (running) pose_active[base + __popc(ballot & ((1u << lane) - 1u))] = k;
+  if (k == kPoseCompactThreads - 1) *pose_count = base + __popc(ballot);
 }
 
 }  // namespace clc

@@ -239,6 +239,29 @@ int clc_information_segments(clc_problem* p, int64_t n_segments, const int64_t* 
 int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, double* poses, const clc_lm_options* opt,
                           clc_lm_summary* summaries, clc_lm_iteration* trace, int trace_cap);
 
+/* One calibration at many poses: K = n_poses poses over ALL frames of the problem, one shared pass over the points per
+ * evaluation or LM iteration (a multi-start from K start poses, or the cost along a grid of poses).  poses[K * 7].
+ * Pose k's row is what clc_eval / clc_solve_lm return at or from poses[k] on the same problem, up to the order of summation;
+ * problems the one-cluster kernel serves (clc_debug_dispatch: CLC_PATH_ONE_CLUSTER, one cluster per pose in one launch) return
+ * those bytes exactly.  Pose k's bytes depend on poses[k] only, not on K or the other poses: a K = 1 call returns the bytes of
+ * that pose's row in a larger call, and permuting the poses permutes the outputs.  Two calls return identical bytes.  Every
+ * loss kind of clc_problem_set_loss, with or without edge residuals, on both kernel families.
+ * Rejected before the device is touched, with CLC_ERR_INVALID: a NULL problem or poses, n_poses outside [1, 1024], a pose entry
+ * that is not finite.  A problem attached to a communicator fails with CLC_ERR_STATE.
+ * Device memory for the length of a call, on problems the sweep kernel serves: about K * (44 * n_frames + 8 * n_edges) doubles
+ * (every pose's frame constants, raw and expanded per-frame rows; 10^5 frames and K = 1024: about 36 GB), a failed allocation
+ * returning CLC_ERR_CUDA.  On problems the one-cluster kernel serves: about 21 KB per start (its LM state with 256 trace rows). */
+/* clc_eval per pose: H36[K * 36] (row-major 6x6) and g6[K * 6] may be NULL; cost[K] may not. */
+int clc_eval_poses(clc_problem* p, int64_t n_poses, const double* poses, double* H36, double* g6, double* cost);
+/* clc_solve_lm from every pose (overwritten with its result), the K solves advancing side by side; a start that has terminated
+ * costs the later iterations nothing.  opt (NULL: defaults) holds for every start.  summaries[K] and trace[K * trace_cap] as
+ * clc_solve_lm_segments' (device_ms: the time of the whole call; num_sweeps: the start's own sweeps; trace_cap in [0, 256]; when
+ * it is 0, the sweep kernel's path allocates no trace memory on the device and the one-cluster path copies no trace rows).  *best (best may be NULL): the index of the lowest final_cost among the starts whose
+ * termination is not CLC_TERM_FAILURE, the lowest index on a tie, -1 when every start failed.  NULL summaries, or a trace_cap
+ * outside [0, 256] or without trace, fail with CLC_ERR_INVALID. */
+int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const clc_lm_options* opt, clc_lm_summary* summaries,
+                        clc_lm_iteration* trace, int trace_cap, int64_t* best);
+
 /* replaces: CamLaserCalClosedSolution(), reference src/LaseCamCalCeres.cpp:112-203.  Tlc16 row-major.
  * AtA81/Atb9 (the 9x9 normal equations) may be NULL. */
 int clc_closed_form(clc_problem* p, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
@@ -384,6 +407,9 @@ int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flu
  * fix-up and the two-level reduction into per-segment sums (clc_eval_segments without the copy to the host). */
 int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, int n, int flush_l2,
                        float* ms_each);
+/* The same for one evaluation of clc_eval_poses on the path it picks: each bracket holds the K poses' frame constants, sweeps,
+ * fix-up and reduction (or the one-cluster launch), not the copy to the host. */
+int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n, int flush_l2, float* ms_each);
 /* The gather of clc_problem_subset(src, keep): `n` times a scratch subset is prepared, its gather kernel is timed alone (CUDA
  * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
  * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
