@@ -93,7 +93,7 @@ class LmOptions(C.Structure):
         ("max_num_consecutive_invalid_steps", C.c_int),
         ("jacobi_scaling", C.c_int),
         ("iterations_per_sync", C.c_int),
-        ("reserved", C.c_int),
+        ("fixed_mask", C.c_int),
     ]
 
 

@@ -236,9 +236,31 @@ def _poses(poses):
     return x, K
 
 
-def default_options(**kw) -> LmOptions:
+FIXED_NAMES = ("tx", "ty", "tz", "rx", "ry", "rz")  # bit k of clc_lm_options.fixed_mask: tangent coordinate k of Plus
+
+
+def fixed_mask(fixed) -> int:
+    """Names of held tangent coordinates -> clc_lm_options.fixed_mask.  tx ty tz: translation of T_cl (camera frame); rx ry
+    rz: the right-multiplied rotation increment (laser frame).  A held rotation name removes that axis from every increment;
+    it does not freeze an Euler angle."""
+    if isinstance(fixed, str):
+        fixed = (fixed,)
+    mask = 0
+    for name in fixed:
+        if name not in FIXED_NAMES:
+            raise ValueError(f"unknown coordinate {name!r}: the names are {' '.join(FIXED_NAMES)}")
+        mask |= 1 << FIXED_NAMES.index(name)
+    if mask == (1 << 6) - 1:
+        raise ValueError("holding all six coordinates leaves nothing to solve")
+    return mask
+
+
+def default_options(fixed=(), **kw) -> LmOptions:
+    """clc_lm_default_options, then the fields in kw.  fixed: names of the tangent coordinates held at the start pose's
+    value in every solve with these options (FIXED_NAMES), e.g. default_options(fixed=("ty", "rx"))."""
     o = LmOptions()
     _lib.load().clc_lm_default_options(C.byref(o))
+    o.fixed_mask = fixed_mask(fixed)
     for k, v in kw.items():
         setattr(o, k, v)
     return o

@@ -763,7 +763,7 @@ void clc_lm_default_options(clc_lm_options* o) {
   o->max_num_consecutive_invalid_steps = 5;
   o->jacobi_scaling = 1;
   o->iterations_per_sync = 8;
-  o->reserved = 0;
+  o->fixed_mask = 0;
 }
 
 void clc_T_to_pose7(const double T[16], double pose7[7]) {
@@ -1522,15 +1522,30 @@ int solve_finish(clc_problem* p, double pose7[7], clc_lm_summary* summary, clc_l
   return CLC_OK;
 }
 
+// the first check of every LM entry point, before its other arguments and any device work
+int check_fixed_mask(const clc_lm_options* opt) {
+  if (opt && (opt->fixed_mask < 0 || opt->fixed_mask >= 63))
+    return fail(CLC_ERR_INVALID, "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)");
+  return CLC_OK;
+}
+
+// the options of every LM entry point (NULL: defaults), checked before any device work
+int lm_options(const clc_lm_options* opt_in, clc_lm_options* opt) {
+  if (opt_in) *opt = *opt_in; else clc_lm_default_options(opt);
+  if (opt->max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
+  int rc = check_fixed_mask(opt);
+  if (rc != CLC_OK) return rc;
+  if (opt->iterations_per_sync < 1) opt->iterations_per_sync = 1;
+  return CLC_OK;
+}
+
 // the whole solve over the shards `ps` (n == 1: a plain problem, possibly one rank of a multi-process job)
 int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_options* opt_in, clc_lm_summary* summary,
               clc_lm_iteration* trace, int trace_cap) {
   clc_lm_options opt;
-  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
-  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
-  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  int rc = lm_options(opt_in, &opt);
+  if (rc != CLC_OK) return rc;
   std::vector<SolveCtx> ctx((size_t)n);
-  int rc = CLC_OK;
   for (int g = 0; g < n && rc == CLC_OK; ++g) rc = solve_begin(ps[g], pose7, opt, &ctx[g]);
   if (rc != CLC_OK) return rc;
   // an abandoned solve (an error below) still demotes the L2 lines its sweeps kept resident; solve_finish does it otherwise
@@ -1616,6 +1631,8 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
 
 int clc_solve_lm(clc_problem* p, double pose7[7], const clc_lm_options* opt_in, clc_lm_summary* summary,
                  clc_lm_iteration* trace, int trace_cap) {
+  const int rc = check_fixed_mask(opt_in);
+  if (rc != CLC_OK) return rc;
   if (!p || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
   return solve_all(&p, 1, pose7, opt_in, summary, trace, trace_cap);
 }
@@ -1779,14 +1796,13 @@ int clc_information_segments(clc_problem* p, int64_t n_segments, const int64_t* 
 
 int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, double* poses, const clc_lm_options* opt_in,
                           clc_lm_summary* summaries, clc_lm_iteration* trace, int trace_cap) {
+  if (check_fixed_mask(opt_in) != CLC_OK) return CLC_ERR_INVALID;
   if (!summaries || trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
     return fail(CLC_ERR_INVALID, "NULL summaries, or trace_cap outside [0, 256] without a trace array");
   int rc = check_segments(p, n_segments, seg_offsets, poses);
   if (rc != CLC_OK) return rc;
   clc_lm_options opt;
-  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
-  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
-  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  if ((rc = lm_options(opt_in, &opt)) != CLC_OK) return rc;
   const int64_t W = n_segments;
   SegmentRun r;
   if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK || (rc = seg_alloc(p, &r.cores, (size_t)W)) != CLC_OK ||
@@ -2017,14 +2033,13 @@ int clc_eval_poses(clc_problem* p, int64_t n_poses, const double* poses, double*
 
 int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const clc_lm_options* opt_in, clc_lm_summary* summaries,
                         clc_lm_iteration* trace, int trace_cap, int64_t* best) {
+  if (check_fixed_mask(opt_in) != CLC_OK) return CLC_ERR_INVALID;
   if (!summaries || trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
     return fail(CLC_ERR_INVALID, "NULL summaries, or trace_cap outside [0, 256] without a trace array");
   int rc = check_poses(p, n_poses, poses);
   if (rc != CLC_OK) return rc;
   clc_lm_options opt;
-  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
-  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
-  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  if ((rc = lm_options(opt_in, &opt)) != CLC_OK) return rc;
   if ((rc = set_device(p)) != CLC_OK) return rc;
   const int64_t K = n_poses;
   const int loss = p->loss_kind;
@@ -2723,6 +2738,7 @@ int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* r
 
 int clc_group_solve_lm(clc_group* g, double pose7[7], const clc_lm_options* opt, clc_lm_summary* summary,
                        clc_lm_iteration* trace, int trace_cap) {
+  if (check_fixed_mask(opt) != CLC_OK) return CLC_ERR_INVALID;
   if (!g || g->problems.empty() || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
   return solve_all(g->problems.data(), (int)g->problems.size(), pose7, opt, summary, trace, trace_cap);
 }

@@ -79,6 +79,30 @@ CLC_HD double gradient_max_norm(const double* x, const double* g) {
   return m;
 }
 
+// Held coordinates (clc_lm_options.fixed_mask): Ceres' LM on the reduced local parameterization.  Each held coordinate leaves
+// the H and g just stored at x: its row and column of H become 0 but for a unit diagonal, its entry of g 0.  Every later use
+// then sees the free coordinates only -- gradient_max_norm (g embedded with zeros), the Jacobi-scaled system and its LM
+// diagonal, whose positive pivot makes the Cholesky step of a held coordinate exactly 0 and that of the free ones the step of
+// the reduced system (every product with a held entry is 0), and the model cost change.  Done in place on the state (shared
+// memory on the device), off the register-resident step code.
+CLC_HD void lm_hold(LmCore* s, int fixed) {
+#pragma unroll 1
+  for (int k = 0; k < 6; ++k) {
+    if (!(fixed >> k & 1)) continue;
+#pragma unroll 1
+    for (int j = 0; j < 6; ++j) s->H[j < k ? tri(j, k) : tri(k, j)] = 0.0;
+    s->H[tri(k, k)] = 1.0;
+    s->g[k] = 0.0;
+  }
+}
+
+// a held translation of the candidate keeps the bits of x (x + 0 would turn a -0.0 into +0.0)
+CLC_HD void lm_hold_cand(LmCore* s, int fixed) {
+#pragma unroll 1
+  for (int k = 0; k < 3; ++k)
+    if (fixed >> k & 1) s->cand[k] = s->x[k];
+}
+
 CLC_HD void lm_record(LmCore* s, clc_lm_iteration* trace, const clc_lm_iteration& it) {
   if (s->n_trace < kTraceMax) trace[s->n_trace] = it;
   s->n_trace++;
@@ -130,6 +154,7 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
     s->x_cost = sums[27];
     for (int i = 0; i < 21; ++i) s->H[i] = sums[i];
     for (int i = 0; i < 6; ++i) s->g[i] = sums[21 + i];
+    if (o.fixed_mask) lm_hold(s, o.fixed_mask);
     for (int k = 0; k < 6; ++k) s->scale[k] = o.jacobi_scaling ? 1.0 / (1.0 + sqrt(s->H[tri(k, k)])) : 1.0;
     s->initial_cost = s->x_cost;
     last.iteration = 0; last.step_is_valid = 1; last.step_is_successful = 1;
@@ -165,6 +190,7 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
       s->x_cost = cand_cost;
       for (int i = 0; i < 21; ++i) s->H[i] = sums[i];
       for (int i = 0; i < 6; ++i) s->g[i] = sums[21 + i];
+      if (o.fixed_mask) lm_hold(s, o.fixed_mask);
       last.step_is_successful = 1;
       last.gradient_max_norm = gradient_max_norm(s->x, s->g);
       const double q = 2.0 * last.relative_decrease - 1.0;
@@ -262,6 +288,7 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
     for (int k = 0; k < 6; ++k) delta[k] = step[k] * s->scale[k];
     CLC_LM_STAMP(5);  // model cost change done
     pose_plus(s->x, delta, s->cand);
+    if (o.fixed_mask) lm_hold_cand(s, o.fixed_mask);
     s->model_cost_change = mcc;
     s->phase = 1;
     CLC_LM_STAMP(6);  // candidate pose done

@@ -110,7 +110,21 @@ typedef struct {
   int max_num_consecutive_invalid_steps; /* 5 */
   int jacobi_scaling;               /* 1 */
   int iterations_per_sync;          /* LM iterations enqueued between host polls of the device `done` flag (8; the first batch of a solve is twice as long) */
-  int reserved;
+  /* Coordinates of the extrinsic held at their start value (0: none).  Bit k holds tangent coordinate k of the reference's
+   * PoseLocalParameterization::Plus: bits 0-2 = dt_x, dt_y, dt_z (translation of T_cl, camera frame), bits 3-5 = dtheta_x,
+   * dtheta_y, dtheta_z (right-multiplied rotation increment, laser frame).  The solve is Ceres' LM on the reduced local
+   * parameterization (a Ceres 2.1 local parameterization of local size 6 - k wrapped around the reference's):
+   *   - Jacobi scaling, the LM diagonal, the Cholesky step, the model cost change and gradient_max_norm use the free
+   *     coordinates only; the parameter tolerance still measures the 7-vector;
+   *   - a held translation coordinate keeps its start value bit for bit;
+   *   - a held rotation bit removes that axis from every increment.  It does NOT freeze an Euler angle: increments about the
+   *     other two axes do not commute, so the orientation about the held axis may still drift as they accumulate.
+   * Typical use: the coordinates the reference's null-space report (clc_information) names as unobservable, held at a value
+   * from a tape measure or a drawing.  A mask with bits above 5, or with all six bits set (63), fails with CLC_ERR_INVALID
+   * before any device work in clc_solve_lm, clc_group_solve_lm, clc_solve_lm_segments and clc_solve_lm_starts.  (This field
+   * was `reserved` and ignored before: callers that left garbage in it now get CLC_ERR_INVALID.)  clc_lm_default_options
+   * sets 0. */
+  int fixed_mask;
 } clc_lm_options;
 
 /* termination codes (Ceres TerminationType + the tolerance that fired) */
