@@ -255,6 +255,37 @@ def fixed_mask(fixed) -> int:
     return mask
 
 
+TIME_OFFSET_NAMES = FIXED_NAMES + ("td",)  # bit 6 of fixed_mask holds td in solve_time_offset only
+
+
+def time_offset_mask(fixed) -> int:
+    """Names of the coordinates solve_time_offset holds (TIME_OFFSET_NAMES: the six of fixed_mask, then "td") -> its
+    fixed_mask, any proper subset of the seven."""
+    if isinstance(fixed, str):
+        fixed = (fixed,)
+    mask = 0
+    for name in fixed:
+        if name not in TIME_OFFSET_NAMES:
+            raise ValueError(f"unknown coordinate {name!r}: the names are {' '.join(TIME_OFFSET_NAMES)}")
+        mask |= 1 << TIME_OFFSET_NAMES.index(name)
+    if mask == (1 << 7) - 1:
+        raise ValueError("holding all seven coordinates leaves nothing to solve")
+    return mask
+
+
+def _trajectory(knot_times, knot_poses, frame_times, n_frames):
+    """The float64 arrays of clc_problem_set_trajectory (checked before any device work: the library checks them too)."""
+    t = np.ascontiguousarray(knot_times, dtype=np.float64)
+    q = np.ascontiguousarray(knot_poses, dtype=np.float64)
+    s = np.ascontiguousarray(frame_times, dtype=np.float64)
+    K = t.shape[0] if t.ndim == 1 else -1
+    if K < 2 or q.shape != (K, 7):
+        raise ValueError(f"knot_times must be [K >= 2] and knot_poses [K, 7], not {t.shape} and {q.shape}")
+    if s.shape != (n_frames,):
+        raise ValueError(f"frame_times must have shape ({n_frames},), not {s.shape}")
+    return t, q, s, K
+
+
 def default_options(fixed=(), **kw) -> LmOptions:
     """clc_lm_default_options, then the fields in kw.  fixed: names of the tangent coordinates held at the start pose's
     value in every solve with these options (FIXED_NAMES), e.g. default_options(fixed=("ty", "rx"))."""
@@ -536,6 +567,52 @@ class Problem:
                   for k in range(K)]
         return x, list(summaries), traces, best.value
 
+    # ---- the camera-laser time offset ----
+    def set_trajectory(self, knot_times, knot_poses, frame_times):
+        """Attach the board trajectory of the time-offset calls (clc_problem_set_trajectory): knot_times [K >= 2] in seconds,
+        strictly increasing; knot_poses [K, 7] in the frame_pose convention (qx qy qz qw tx ty tz of T_ca); frame_times
+        [n_frames], every frame's scan time on the laser clock.  None for the three arguments removes it.  subset and trim
+        results carry no trajectory."""
+        if knot_times is None and knot_poses is None and frame_times is None:
+            _lib.check(self._L.clc_problem_set_trajectory(self._h, 0, None, None, None), "clc_problem_set_trajectory")
+            return
+        t, q, s, K = _trajectory(knot_times, knot_poses, frame_times, self.sizes()[0])
+        _lib.check(self._L.clc_problem_set_trajectory(self._h, K, _dp(t), _dp(q), _dp(s)), "clc_problem_set_trajectory")
+
+    def eval_time_offset(self, pose7, td):
+        """eval() with the time offset td: the planes interpolated at every frame's scan time + td (clc_eval_time_offset).
+        Returns (cost, H [7, 7], g [7]) over (tx ty tz rx ry rz td)."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        H, g, cost = np.empty((7, 7)), np.empty(7), C.c_double()
+        _lib.check(self._L.clc_eval_time_offset(self._h, _dp(pose7), float(td), _dp(H), _dp(g), C.byref(cost)),
+                   "clc_eval_time_offset")
+        return cost.value, H, g
+
+    def information_time_offset(self, pose7, td):
+        """information() with the time offset td (clc_information_time_offset): (H [7, 7], b [7], chi, sv [7]); the right
+        singular vectors go to self.last_V [7, 7].  A ~0 singular value whose V column is +-e_td: the board never moved."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        H, b, sv, chi = np.empty((7, 7)), np.empty(7), np.empty(7), C.c_double()
+        self.last_V = np.empty((7, 7))
+        _lib.check(self._L.clc_information_time_offset(self._h, _dp(pose7), float(td), _dp(H), _dp(b), C.byref(chi), _dp(sv),
+                                                       _dp(self.last_V)), "clc_information_time_offset")
+        return H, b, chi.value, sv
+
+    def solve_time_offset(self, pose7, td=0.0, options: LmOptions | None = None, fixed=None, trace_cap=256):
+        """solve() of the extrinsic and the time offset td together (clc_solve_lm_time_offset).  fixed: names of
+        TIME_OFFSET_NAMES held at their start values for this call (overrides options.fixed_mask); e.g. fixed=("tx", "ty", "tz",
+        "rx", "ry", "rz") estimates the offset alone, fixed="td" the extrinsic alone.  Returns (pose7, td, summary, trace)."""
+        x = np.ascontiguousarray(pose7, dtype=np.float64).copy()
+        t = C.c_double(float(td))
+        o = LmOptions.from_buffer_copy(options) if options is not None else default_options()  # the caller's stays as it is
+        if fixed is not None:
+            o.fixed_mask = time_offset_mask(fixed)
+        s = LmSummary()
+        tr = (LmIteration * trace_cap)() if trace_cap > 0 else None
+        _lib.check(self._L.clc_solve_lm_time_offset(self._h, _dp(x), C.byref(t), C.byref(o), C.byref(s), tr, int(trace_cap)),
+                   "clc_solve_lm_time_offset")
+        return x, t.value, s, [tr[i] for i in range(min(s.num_iterations, trace_cap))] if trace_cap > 0 else []
+
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()
         _lib.check(self._L.clc_closed_form(self._h, _dp(T), C.byref(un), _dp(AtA), _dp(Atb)), "clc_closed_form")
@@ -586,6 +663,15 @@ class Problem:
         x, K = _poses(poses)
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_poses(self._h, K, _dp(x), int(n), int(bool(flush_l2)), ms), "clc_bench_poses")
+        return np.array(ms[:], dtype=np.float64)
+
+    def bench_time_offset(self, pose7, td, n, flush_l2=True):
+        """Device time of n time-offset iterations (planes and constants, segment sweep, fix-up, two-level reduction;
+        clc_bench_time_offset), ms each."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_time_offset(self._h, _dp(pose7), float(td), int(n), int(bool(flush_l2)), ms),
+                   "clc_bench_time_offset")
         return np.array(ms[:], dtype=np.float64)
 
     def bench_subset(self, keep, n, flush_l2=True):

@@ -28,6 +28,7 @@
 #include "clc_small.cuh"
 #include "clc_subset.cuh"
 #include "clc_subset_plan.h"
+#include "clc_time_offset.cuh"
 #include "clc_trim.cuh"
 
 namespace {
@@ -296,6 +297,10 @@ struct clc_problem {
   bool planar = false;         // the two-stream kernels are in use (z_all_zero && planar_mode != 0 && large enough)
   int planar_mode = 1;         // 1 = automatic (default), 0 = always the general three-stream kernels
   int64_t planar_min_points = 0;
+  // board trajectory of the time-offset calls (clc_problem_set_trajectory; subsets and trims carry none): one block of
+  // knot times [K] and frame times [n_frames] (both relative to the first knot), knots [K * kKnotDoubles], w [(K - 1) * 3]
+  double* traj = nullptr;
+  int64_t traj_knots = 0;
 };
 
 namespace {
@@ -789,7 +794,7 @@ int clc_problem_destroy(clc_problem* p) {
   if (p->stream) cudaStreamSynchronize(p->stream);
   if (p->stream) {
     void* bufs[] = {p->xy_block, p->z_block, p->d_nonplanar, p->frame_pose, p->frame_pose_true, p->plane, p->offsets, p->warp_first_frame, p->edge_plane, p->edge_pt,
-                    p->partials_ll, p->sums, p->pose, p->launch_seq, p->pose_ll, p->lm, p->flush_buf, p->p2p_error};
+                    p->partials_ll, p->sums, p->pose, p->launch_seq, p->pose_ll, p->lm, p->flush_buf, p->p2p_error, p->traj};
     for (void* b : bufs)
       if (b) cudaFreeAsync(b, p->stream);  // back to the device's memory pool: re-creating a problem is cheap
     cudaStreamSynchronize(p->stream);
@@ -1687,8 +1692,9 @@ int seg_alloc_bytes(clc_problem* p, void** out, size_t bytes) {
 }
 #define seg_alloc(p, out, n) seg_alloc_bytes((p), reinterpret_cast<void**>(out), sizeof(**(out)) * (size_t)(n))
 
-// the plan, the work buffers and the problem's eval pose (which the sweep does not use) on the device
-int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, SegmentRun* r) {
+// the plan, the work buffers and the problem's eval pose (which the sweep does not use) on the device; rows and partials are
+// `width` doubles wide (the time-offset calls expand every frame into kTdSums)
+int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, SegmentRun* r, int width = clc::kNumSums) {
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   r->p = p;
@@ -1699,9 +1705,9 @@ int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, Segm
   if ((rc = seg_alloc(p, &r->frame_seg, N)) != CLC_OK || (rc = seg_alloc(p, &r->chunk_offsets, plan.chunk_offsets.size())) != CLC_OK ||
       (rc = seg_alloc(p, &r->seg_chunks, plan.seg_chunks.size())) != CLC_OK ||
       (rc = seg_alloc(p, &r->consts, (N + (size_t)p->n_edges) * 4)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->raw, N * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->rows, N * clc::kNumSums)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->raw, N * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->rows, N * width)) != CLC_OK ||
       (rc = seg_alloc(p, &r->slots, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->partials, (size_t)r->n_chunks * clc::kNumSums)) != CLC_OK)
+      (rc = seg_alloc(p, &r->partials, (size_t)r->n_chunks * width)) != CLC_OK)
     return rc;
   // pageable sources: each copy has read its source when it returns
   if (N > 0) CLC_CUDA(cudaMemcpyAsync(r->frame_seg, plan.frame_seg.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice, p->stream));
@@ -1861,6 +1867,271 @@ int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg
     const int n = std::min(c.n_trace, trace_cap);
     for (int i = 0; i < n; ++i) trace[s * trace_cap + i] = rows[(size_t)s * trace_cap + i];
   }
+  return CLC_OK;
+}
+
+// ---- the camera-laser time offset (clc_time_offset.cuh) ---------------------------------------------------------------
+// Every problem size runs it on the sweep kernel K1 (kModeSegments) with the kernel family eval uses, as one segment of all frames:
+// segments_prepare's plan and buffers with seg_offsets = {0, n_frames}, rows and partials kTdSums wide.
+
+namespace {
+
+clc::TrajView traj_view(const clc_problem* p) {
+  const int64_t K = p->traj_knots;
+  return clc::TrajView{p->traj, p->traj + K + p->n_frames, p->traj + K + p->n_frames + K * clc::kKnotDoubles, K};
+}
+
+// rejects bad arguments before the device is touched (pose7 and td: the point of an evaluation, or the start of a solve)
+int check_time_offset(const clc_problem* p, const double* pose7, const double* td) {
+  if (!p || !pose7 || !td) return fail(CLC_ERR_INVALID, "NULL argument");
+  if (p->n_edges > 0) return fail(CLC_ERR_INVALID, "time-offset calls take a problem without edge residuals");
+  if (p->comm_obj != nullptr || p->nranks > 1) return fail(CLC_ERR_STATE, "time-offset calls run on a problem without a communicator");
+  if (p->traj == nullptr) return fail(CLC_ERR_STATE, "the problem has no trajectory (clc_problem_set_trajectory)");
+  for (int i = 0; i < 7; ++i)
+    if (!clc::is_finite(pose7[i])) return fail(CLC_ERR_INVALID, "a pose7 entry is not finite");
+  if (!clc::is_finite(*td)) return fail(CLC_ERR_INVALID, "td is not finite");
+  return CLC_OK;
+}
+
+// The device buffers of one time-offset call: SegmentRun over one segment of every frame (poses: the point (pose7, td) of an
+// evaluation, sums: its kTdSums sums), plus n, mdot, cdot of every frame and the solve's LM state.
+struct TimeRun {
+  SegmentRun s;
+  double* tframe = nullptr;         // [n_frames * kTdFrameDoubles]
+  clc::LmCoreTd* core = nullptr;    // solve
+  ~TimeRun() {
+    if (!s.p) return;
+    cudaSetDevice(s.p->device);
+    for (void* b : {(void*)tframe, (void*)core})
+      if (b) cudaFreeAsync(b, s.p->stream);
+  }
+};
+
+int time_prepare(clc_problem* p, TimeRun* r) {
+  const int64_t off[2] = {0, p->n_frames};
+  int rc;
+  if ((rc = segments_prepare(p, 1, off, &r->s, clc::kTdSums)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->tframe, (size_t)p->n_frames * clc::kTdFrameDoubles)) != CLC_OK)
+    return rc;
+  return CLC_OK;
+}
+
+// One iteration at pose8 = (pose7, td) on the device.  sums: [kTdSums] or nullptr; core: the solve's LM state (lm_update_td runs on
+// it), with its trace and `done` flag.
+int time_iteration(const TimeRun& r, int loss, const double* pose8, double* sums, clc::LmCoreTd* core, clc_lm_iteration* trace,
+                   int trace_cap, int* done) {
+  clc_problem* p = r.s.p;
+  const clc::ProblemView v = make_view(p);
+  const clc::TrajView tv = traj_view(p);
+  const double* frame_time = p->traj + p->traj_knots;
+  const int threads = 256;
+  if (p->n_frames > 0) {
+    const unsigned fb = (unsigned)((p->n_frames + threads - 1) / threads);
+    clc::clc_time_consts_kernel<<<fb, threads, 0, p->stream>>>(v, tv, frame_time, pose8, done, r.s.consts, r.tframe);
+    CLC_LAUNCH_CHECK();
+    int rc = launch_sweep(p, clc::kModeSegments, loss, false, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
+                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw, r.s.slots, r.s.consts);
+    if (rc != CLC_OK) return rc;
+    void (*fixup)(clc::ProblemView, const double*, const double*, const int*, const double*, const double*, double*) =
+        loss == clc::kLossCauchy  ? clc::clc_time_fixup_kernel<clc::kLossCauchy>
+        : loss == clc::kLossHuber ? clc::clc_time_fixup_kernel<clc::kLossHuber>
+        : loss == clc::kLossSoftL1 ? clc::clc_time_fixup_kernel<clc::kLossSoftL1>
+                                   : clc::clc_time_fixup_kernel<clc::kLossNone>;
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.s.consts, r.tframe, done, r.s.raw, r.s.slots, r.s.rows);
+    CLC_LAUNCH_CHECK();
+  }
+  if (r.s.n_chunks > 0) {
+    const unsigned cb = (unsigned)((r.s.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+    clc::clc_time_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.rows, r.s.chunk_offsets, r.s.n_chunks, done,
+                                                                                  r.s.partials);
+    CLC_LAUNCH_CHECK();
+  }
+  clc::clc_time_lm_kernel<<<1, 32, 0, p->stream>>>(r.s.partials, r.s.n_chunks, sums, core, trace, trace_cap, done);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the point (pose7, td) and the sum buffers of an evaluation on the device
+int time_eval_prepare(clc_problem* p, const double* pose7, double td, TimeRun* r) {
+  int rc;
+  if ((rc = time_prepare(p, r)) != CLC_OK || (rc = seg_alloc(p, &r->s.poses, 8)) != CLC_OK ||
+      (rc = seg_alloc(p, &r->s.sums, clc::kTdSums)) != CLC_OK)
+    return rc;
+  double x8[8];
+  for (int i = 0; i < 7; ++i) x8[i] = pose7[i];
+  x8[7] = td;
+  CLC_CUDA(cudaMemcpyAsync(r->s.poses, x8, sizeof(x8), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));  // x8 is pageable and on this stack frame
+  return CLC_OK;
+}
+
+// the kTdSums sums at (pose7, td) (which: 0 eval with the problem's loss, 1 information -- no loss)
+int time_eval_run(clc_problem* p, const double* pose7, double td, int which, double* sums) {
+  int rc = check_time_offset(p, pose7, &td);
+  if (rc != CLC_OK) return rc;
+  TimeRun r;
+  if ((rc = time_eval_prepare(p, pose7, td, &r)) != CLC_OK) return rc;
+  rc = time_iteration(r, which == 0 ? p->loss_kind : clc::kLossNone, r.s.poses, r.s.sums, nullptr, nullptr, 0, nullptr);
+  if (rc != CLC_OK) return rc;
+  CLC_CUDA(cudaMemcpyAsync(sums, r.s.sums, sizeof(double) * clc::kTdSums, cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  return CLC_OK;
+}
+
+void unpack_H7(const double* sums, double* H49) {
+  for (int i = 0; i < 7; ++i)
+    for (int j = i; j < 7; ++j) H49[i * 7 + j] = H49[j * 7 + i] = sums[clc::tri7(i, j)];
+}
+
+}  // namespace
+
+int clc_problem_set_trajectory(clc_problem* p, int64_t n_knots, const double* knot_times, const double* knot_poses,
+                               const double* frame_times) {
+  if (!p) return fail(CLC_ERR_INVALID, "NULL problem");
+  const int64_t K = n_knots, N = p->n_frames;
+  if (K < 0 || K == 1) return fail(CLC_ERR_INVALID, "n_knots must be 0 (no trajectory) or at least 2");
+  if (K > 0) {
+    if (!knot_times || !knot_poses || !frame_times) return fail(CLC_ERR_INVALID, "NULL knot_times, knot_poses or frame_times");
+    for (int64_t k = 0; k < K; ++k) {
+      if (!clc::is_finite(knot_times[k])) return fail(CLC_ERR_INVALID, "a knot_times entry is not finite");
+      if (k > 0 && !(knot_times[k] > knot_times[k - 1])) return fail(CLC_ERR_INVALID, "knot_times must be strictly increasing");
+    }
+    for (int64_t i = 0; i < 7 * K; ++i)
+      if (!clc::is_finite(knot_poses[i])) return fail(CLC_ERR_INVALID, "a knot_poses entry is not finite");
+    for (int64_t k = 0; k < K; ++k) {
+      const double* q = knot_poses + 7 * k;
+      if (q[0] == 0.0 && q[1] == 0.0 && q[2] == 0.0 && q[3] == 0.0) return fail(CLC_ERR_INVALID, "a knot_poses quaternion is zero");
+    }
+    for (int64_t f = 0; f < N; ++f)
+      if (!clc::is_finite(frame_times[f])) return fail(CLC_ERR_INVALID, "a frame_times entry is not finite");
+    if (p->n_edges > 0) return fail(CLC_ERR_INVALID, "time-offset calls take a problem without edge residuals");
+  }
+  if (p->comm_obj != nullptr || p->nranks > 1) return fail(CLC_ERR_STATE, "time-offset calls run on a problem without a communicator");
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  if (p->traj) {
+    CLC_CUDA(cudaFreeAsync(p->traj, p->stream));
+    p->traj = nullptr;
+    p->traj_knots = 0;
+  }
+  if (K == 0) return CLC_OK;
+  // times relative to the first knot, subtracted once in double (exact for nearby epoch stamps, by Sterbenz)
+  std::vector<double> h((size_t)(K + N + K * clc::kKnotDoubles + (K - 1) * 3));
+  double* t = h.data();
+  double* s = t + K;
+  double* knot = s + N;
+  double* omega = knot + K * clc::kKnotDoubles;
+  for (int64_t k = 0; k < K; ++k) t[k] = knot_times[k] - knot_times[0];
+  for (int64_t f = 0; f < N; ++f) s[f] = frame_times[f] - knot_times[0];
+  for (int64_t k = 0; k < K; ++k) clc::traj_knot(knot_poses + 7 * k, knot + k * clc::kKnotDoubles);
+  for (int64_t k = 0; k + 1 < K; ++k)
+    clc::traj_omega(knot + k * clc::kKnotDoubles, knot + (k + 1) * clc::kKnotDoubles, omega + 3 * k);
+  CLC_CUDA(cudaMallocAsync(&p->traj, sizeof(double) * h.size(), p->stream));
+  CLC_CUDA(cudaMemcpyAsync(p->traj, h.data(), sizeof(double) * h.size(), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  p->traj_knots = K;
+  return CLC_OK;
+}
+
+int clc_eval_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double g7[7], double* cost) {
+  double sums[clc::kTdSums];
+  const int rc = time_eval_run(p, pose7, td, 0, sums);
+  if (rc != CLC_OK) return rc;
+  if (H49) unpack_H7(sums, H49);
+  if (g7) for (int i = 0; i < 7; ++i) g7[i] = sums[28 + i];
+  if (cost) *cost = sums[35];
+  return CLC_OK;
+}
+
+int clc_information_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double b7[7], double* chi,
+                                double singular_values7[7], double V49[49]) {
+  double sums[clc::kTdSums];
+  const int rc = time_eval_run(p, pose7, td, 1, sums);
+  if (rc != CLC_OK) return rc;
+  double H[49];
+  unpack_H7(sums, H);
+  if (H49) std::memcpy(H49, H, sizeof(H));
+  if (b7) for (int i = 0; i < 7; ++i) b7[i] = -sums[28 + i];
+  if (chi) *chi = 2.0 * sums[35];
+  if (singular_values7 || V49) {
+    double w[7], V[49];
+    sym_eig<7>(H, w, V);
+    int order[7] = {0, 1, 2, 3, 4, 5, 6};
+    std::sort(order, order + 7, [&](int a, int b) { return std::fabs(w[a]) > std::fabs(w[b]); });
+    for (int c = 0; c < 7; ++c) {
+      if (singular_values7) singular_values7[c] = std::fabs(w[order[c]]);
+      if (V49)
+        for (int r = 0; r < 7; ++r) V49[r * 7 + c] = V[r * 7 + order[c]];
+    }
+  }
+  return CLC_OK;
+}
+
+int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const clc_lm_options* opt_in, clc_lm_summary* summary,
+                             clc_lm_iteration* trace, int trace_cap) {
+  if (opt_in && (opt_in->fixed_mask < 0 || opt_in->fixed_mask >= 127))
+    return fail(CLC_ERR_INVALID, "fixed_mask must hold a proper subset of the seven coordinates (0 <= mask < 127)");
+  if (trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
+    return fail(CLC_ERR_INVALID, "trace_cap outside [0, 256], or without a trace array");
+  int rc = check_time_offset(p, pose7, td);
+  if (rc != CLC_OK) return rc;
+  clc_lm_options opt;
+  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
+  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
+  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  TimeRun r;
+  if ((rc = time_prepare(p, &r)) != CLC_OK || (rc = seg_alloc(p, &r.core, 1)) != CLC_OK ||
+      (rc = seg_alloc(p, &r.s.counters, 1)) != CLC_OK)
+    return rc;
+  if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, trace_cap)) != CLC_OK) return rc;
+  clc::LmCoreTd core;
+  clc::lm_init_td(&core, pose7, *td, opt);
+  CLC_CUDA(cudaMemcpyAsync(r.core, &core, sizeof(core), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemsetAsync(r.s.counters, 0, sizeof(int), p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));  // core is pageable and on this stack frame
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+  const int loss = p->loss_kind;
+  const double* cand = r.core->cand;  // (pose7, td) of the next sweep
+  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
+  const int max_sweeps = opt.max_num_iterations + 2;
+  int launched = 0;
+  while (launched < max_sweeps) {
+    // the first batch is twice as long, as in solve_all
+    const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
+    for (int i = 0; i < batch; ++i) {
+      rc = time_iteration(r, loss, cand, nullptr, r.core, r.s.trace, trace_cap, r.s.counters);
+      if (rc != CLC_OK) return rc;
+    }
+    launched += batch;
+    CLC_CUDA(cudaMemcpyAsync(p->h_done, r.s.counters, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(sync_stream_low_latency(p->stream));
+    if (*p->h_done != 0) break;
+  }
+  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+  std::vector<clc_lm_iteration> rows((size_t)trace_cap);
+  CLC_CUDA(cudaMemcpyAsync(&core, r.core, sizeof(core), cudaMemcpyDeviceToHost, p->stream));
+  if (trace_cap > 0)
+    CLC_CUDA(cudaMemcpyAsync(rows.data(), r.s.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  float ms = 0.f;
+  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
+  for (int i = 0; i < 7; ++i) pose7[i] = core.x[i];  // the last accepted point, as clc_solve_lm
+  *td = core.x[7];
+  if (summary) {
+    summary->termination = core.done ? core.done : CLC_TERM_NO_CONVERGENCE;
+    summary->num_iterations = core.n_trace;
+    summary->num_successful_steps = core.num_successful;
+    summary->num_unsuccessful_steps = core.num_unsuccessful;
+    summary->num_sweeps = core.sweeps;
+    summary->reserved = 0;
+    summary->initial_cost = core.initial_cost;
+    summary->final_cost = core.x_cost;
+    summary->device_ms = ms;
+  }
+  const int n = std::min(core.n_trace, trace_cap);
+  for (int i = 0; i < n; ++i) trace[i] = rows[(size_t)i];
   return CLC_OK;
 }
 
@@ -3461,6 +3732,21 @@ int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_of
   const bool edges = p->n_edges > 0;
   return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
     return segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
+  });
+}
+
+int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int n, int flush_l2, float* ms_each) {
+  if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_time_offset(p, pose7, &td);
+  if (rc != CLC_OK) return rc;
+  TimeRun r;
+  if ((rc = time_eval_prepare(p, pose7, td, &r)) != CLC_OK) return rc;
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
+  const int loss = p->loss_kind;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
+    return time_iteration(r, loss, r.s.poses, r.s.sums, nullptr, nullptr, 0, nullptr);
   });
 }
 

@@ -78,28 +78,40 @@ __device__ __forceinline__ void segment_row_write(const ProblemView& pv, const d
   for (int k = 0; k < kNumSums; ++k) row[k] = out[k];
 }
 
-// Expansion of frame f after a kModeSegments or kModePoses sweep, clc_frame_fixup_kernel's sibling.  An empty frame gets a row of
-// zeros; a whole frame's raw row (kSegRawDoubles), or a split frame's pieces added in warp order, are expanded at the pose of
-// `consts`.
+// The summed moments S[10] and cost_term (as expand_lm takes them) of frame f after a kModeSegments or kModePoses sweep: a whole
+// frame's raw row (kSegRawDoubles), or a split frame's pieces added in warp order.  false, with S and cost_term untouched, for an
+// empty frame.
 template <int LOSS>
-__device__ __forceinline__ void segment_fixup_frame(const ProblemView& pv, const double* __restrict__ consts, int edges, int64_t f,
-                                                    const double* __restrict__ raw, const double* __restrict__ slots,
-                                                    double* __restrict__ rows) {
+__device__ __forceinline__ bool segment_frame_moments(const ProblemView& pv, int64_t f, const double* __restrict__ raw,
+                                                      const double* __restrict__ slots, double* S, double* cost_term) {
   const int64_t fs = pv.offsets[f], fe = pv.offsets[f + 1];
-  double* row = rows + f * kNumSums;
-  if (fe <= fs) {
-    for (int k = 0; k < kNumSums; ++k) row[k] = 0.0;
-    return;
-  }
+  if (fe <= fs) return false;
   int64_t w0, w1;
   frame_warps(fs, fe, pv.per_warp, &w0, &w1);
-  double S[10] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-  double cost_term = 0.0;
+#pragma unroll
+  for (int k = 0; k < 10; ++k) S[k] = 0.0;
+  double ct = 0.0;
   for (int64_t w = w0; w <= w1; ++w) {
     const double* s = w0 == w1 ? raw + f * kSegRawDoubles : slots + frame_slot(w, w0);
 #pragma unroll
     for (int k = 0; k < 10; ++k) S[k] += s[k];
-    cost_term += LOSS == kLossCauchy ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[10];
+    ct += LOSS == kLossCauchy ? log(s[10]) + s[11] * 0.693147180559945309417232121458 : s[10];
+  }
+  *cost_term = ct;
+  return true;
+}
+
+// Expansion of frame f after a kModeSegments or kModePoses sweep, clc_frame_fixup_kernel's sibling.  An empty frame gets a row of
+// zeros; the frame's summed moments (segment_frame_moments) are expanded at the pose of `consts`.
+template <int LOSS>
+__device__ __forceinline__ void segment_fixup_frame(const ProblemView& pv, const double* __restrict__ consts, int edges, int64_t f,
+                                                    const double* __restrict__ raw, const double* __restrict__ slots,
+                                                    double* __restrict__ rows) {
+  double* row = rows + f * kNumSums;
+  double S[10], cost_term;
+  if (!segment_frame_moments<LOSS>(pv, f, raw, slots, S, &cost_term)) {
+    for (int k = 0; k < kNumSums; ++k) row[k] = 0.0;
+    return;
   }
   segment_row_write(pv, consts, f, S, cost_term, LOSS, edges != 0, row);
 }

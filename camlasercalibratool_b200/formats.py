@@ -17,7 +17,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .api import CamLaserCalClosedSolution, CamLaserCalibration, Oberserve, Problem, default_options
+from .api import CamLaserCalClosedSolution, CamLaserCalibration, Oberserve, Problem, T_to_pose7, default_options, pose7_to_T
 
 
 @dataclass
@@ -229,13 +229,14 @@ def select_keyframes(tagpose, dist_min=0.20, theta_min=3.1415926 * 10 / 180.0):
     return sparse
 
 
-def observations_from_segments(tagpose, scans, max_dt=0.02, lines=None):
+def observations_from_segments(tagpose, scans, max_dt=0.02, lines=None, return_times=False):
     """reference main/calibr_offline.cpp:84-155: ``scans`` = [(timestamp, points[n,3])] are the laser segments on the
     board (the output of AutoGetLinePts).  Every scan is matched to the nearest tag pose (accepted within 20 ms), its
     line is fitted by LineFittingCeres -- here for all accepted scans in ONE batched GPU call -- and the two end points
-    on the fitted line become points_on_line.  Returns list[Oberserve]."""
+    on the fitted line become points_on_line.  Returns list[Oberserve]; with return_times, (list[Oberserve], the matched
+    scans' own timestamps [len(obs)])."""
     ts_pose = np.array([p.timestamp for p in tagpose])
-    picked = []
+    picked, times = [], []
     for ts, pts in scans:
         pts = np.asarray(pts, dtype=float).reshape(-1, 3)
         if len(pts) == 0:
@@ -243,8 +244,9 @@ def observations_from_segments(tagpose, scans, max_dt=0.02, lines=None):
         k = int(np.argmin(np.abs(ts_pose - ts)))  # :105-115
         if abs(ts_pose[k] - ts) < max_dt:
             picked.append((tagpose[k], pts))
+            times.append(float(ts))
     if not picked:
-        return []
+        return ([], np.empty(0)) if return_times else []
     if lines is None:
         off = np.concatenate([[0], np.cumsum([len(p) for _, p in picked])])
         fp = np.tile([0, 0, 0, 1, 0, 0, 1.0], (len(picked), 1))
@@ -263,16 +265,37 @@ def observations_from_segments(tagpose, scans, max_dt=0.02, lines=None):
         qca = quat_inverse(pose.qwc)  # :145
         tca = -quat_to_rot(qca) @ pose.twc  # :146
         obs.append(Oberserve(qca, tca, pts, np.array([[x_s, y_s, 0.0], [x_e, y_e, 0.0]])))
-    return obs
+    return (obs, np.array(times)) if return_times else obs
 
 
-def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=None):
+def board_trajectory(tagpose):
+    """Every tag pose as a trajectory knot of Problem.set_trajectory: (times [K], poses [K, 7] in the frame_pose convention),
+    converted as observations_from_segments converts the matched ones (:145-146), in time order; of several poses with the same
+    timestamp the first is kept."""
+    order = sorted(range(len(tagpose)), key=lambda i: tagpose[i].timestamp)
+    times, poses = [], []
+    for i in order:
+        p = tagpose[i]
+        if times and p.timestamp <= times[-1]:
+            continue
+        qca = quat_inverse(p.qwc)
+        poses.append(np.concatenate([qca, -quat_to_rot(qca) @ p.twc]))
+        times.append(float(p.timestamp))
+    return np.array(times), np.array(poses).reshape(-1, 7)
+
+
+def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=None, time_offset=False):
     """reference main/calibr_offline.cpp:52-197 without the rosbag: returns (Tlc, report) or (None, reason).  fixed: names of
     tangent coordinates of T_cl (api.FIXED_NAMES) held at the closed form's value in the LM solve, e.g. the unobservable
-    directions a previous report named."""
+    directions a previous report named.
+    time_offset: after that solve, estimate the camera-laser time offset together with the extrinsic (Problem.solve_time_offset)
+    on the same problem, from the LM result and td = 0, with every tag pose as the board trajectory and the matched scans' own
+    timestamps.  Tlc is then the joint solve's; the report adds time_offset (seconds added to a laser stamp to put it on the
+    camera clock), time_offset_singular_values (information_time_offset's, at the result), time_offset_summary and
+    Tlc_without_time_offset."""
     if len(tagpose) < 10:  # :55-59
         return None, "apriltag pose less than 10."
-    obs = observations_from_segments(select_keyframes(tagpose), scans)
+    obs, scan_times = observations_from_segments(select_keyframes(tagpose), scans, return_times=True)
     if len(obs) < 5:  # :158-163
         return None, "Valid Calibra Data Less"
     Tlc0 = np.eye(4)
@@ -280,6 +303,16 @@ def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=Non
     Tcl = np.linalg.inv(Tlc0)
     options = default_options(fixed=fixed) if fixed else None
     report = CamLaserCalibration(obs, Tcl, False, verbose=verbose, options=options)  # :169-170
+    if time_offset:
+        report["Tlc_without_time_offset"] = np.linalg.inv(Tcl)
+        knot_times, knot_poses = board_trajectory(tagpose)
+        with Problem.from_observations(obs, use_linefitting_data=False) as p:
+            p.set_trajectory(knot_times, knot_poses, scan_times)
+            x, td, summary, _ = p.solve_time_offset(T_to_pose7(Tcl), 0.0, options, trace_cap=0)
+            report["time_offset_singular_values"] = p.information_time_offset(x, td)[3]
+        Tcl = pose7_to_T(x)
+        report["time_offset"] = td
+        report["time_offset_summary"] = summary
     Tlc = np.linalg.inv(Tcl)
     if result_yaml is not None:
         write_result_yaml(result_yaml, Tlc)

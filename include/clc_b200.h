@@ -122,8 +122,8 @@ typedef struct {
    * Typical use: the coordinates the reference's null-space report (clc_information) names as unobservable, held at a value
    * from a tape measure or a drawing.  A mask with bits above 5, or with all six bits set (63), fails with CLC_ERR_INVALID
    * before any device work in clc_solve_lm, clc_group_solve_lm, clc_solve_lm_segments and clc_solve_lm_starts.  (This field
-   * was `reserved` and ignored before: callers that left garbage in it now get CLC_ERR_INVALID.)  clc_lm_default_options
-   * sets 0. */
+   * was `reserved` and ignored before: callers that left garbage in it now get CLC_ERR_INVALID.)  clc_solve_lm_time_offset
+   * alone also takes bit 6 (the time offset td; masks 0..126).  clc_lm_default_options sets 0. */
   int fixed_mask;
 } clc_lm_options;
 
@@ -276,6 +276,49 @@ int clc_eval_poses(clc_problem* p, int64_t n_poses, const double* poses, double*
 int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const clc_lm_options* opt, clc_lm_summary* summaries,
                         clc_lm_iteration* trace, int trace_cap, int64_t* best);
 
+/* ---- the camera-laser time offset ------------------------------------------------------------------------------------------
+ * Every other call takes frame f's board plane as exactly the one of its camera frame.  A scan is matched to the nearest camera
+ * frame, and camera and laser stamps come from different clocks, so while the board moves that plane is off by the motion over the
+ * quantisation error plus a constant clock offset -- a bias no amount of data averages out.  These calls estimate the offset td
+ * (what is added to a laser time to put it on the camera clock) together with the extrinsic, from a board trajectory:
+ *   - K >= 2 knots: times t_k (seconds, strictly increasing) and board poses in the frame_pose convention (qx qy qz qw tx ty tz of
+ *     T_ca).  The library takes T_ac = T_ca^-1 with the normalised quaternion, and times relative to t_0 (subtracted once in
+ *     double, exact for epoch stamps);
+ *   - one scan time s_f per frame: frame f is evaluated at tau_f = s_f + td;
+ *   - on [t_k, t_k+1) (the last interval includes its right end): t_ac lerped, q_ac = q_k (x) Exp(u w_k), u = (tau - t_k) / D_k,
+ *     w_k = Log(q_k^-1 (x) q_k+1) on the shortest arc; outside [t_0, t_{K-1}] the end knot's pose, whose derivative is 0 (such a
+ *     frame constrains T_cl and says nothing about td);
+ *   - the plane n = R_ac^T e_z, d = t_ac,z (at a knot: frame_plane of that knot, up to rounding); the residual e = m.p + c as
+ *     everywhere, scaled by 1/sqrt(#points), with the problem's loss; the Jacobian gains the column de/dtd.
+ * H49 / V49 are row-major 7x7 over (tx ty tz rx ry rz td), g7 / b7 likewise.  Every problem size runs on the sweep kernel K1;
+ * two calls return identical bytes.  Edge residuals are not modelled.
+ * Rejected before the device is touched, with CLC_ERR_INVALID: a NULL problem or output-less argument (pose7, td), a problem with
+ * edge residuals, a pose7 entry or td that is not finite; with CLC_ERR_STATE: a problem attached to a communicator, a problem
+ * without a trajectory. */
+/* Attaches the trajectory (n_knots >= 2: knot_times[n_knots], knot_poses[n_knots * 7], frame_times[n_frames]), replacing any
+ * earlier one, or removes it (n_knots == 0; the arrays are then ignored).  The library keeps its own copy on the device (about
+ * 8 (11 K + n_frames) bytes), freed by clc_problem_destroy.  clc_problem_subset and clc_problem_trim results carry no trajectory.
+ * CLC_ERR_INVALID, leaving p unchanged: n_knots < 0 or == 1, a NULL array, knot times that are not finite or not strictly
+ * increasing, a knot pose entry that is not finite or a zero quaternion, a frame time that is not finite, a problem with edge
+ * residuals; CLC_ERR_STATE: a problem attached to a communicator. */
+int clc_problem_set_trajectory(clc_problem* p, int64_t n_knots, const double* knot_times, const double* knot_poses,
+                               const double* frame_times);
+/* clc_eval with td: H49, g7 (may be NULL) and *cost (may be NULL) at (pose7, td). */
+int clc_eval_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double g7[7], double* cost);
+/* clc_information with td (no loss): H49, b7 = -g, chi, the singular values of H (descending) and the matching right singular
+ * vectors as the columns of V49 -- the observability of td: a board that never moved gives a zero singular value whose V column
+ * is +-e_td.  Any output may be NULL. */
+int clc_information_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double b7[7], double* chi,
+                                double singular_values7[7], double V49[49]);
+/* clc_solve_lm on two parameter blocks: the pose (the reference's PoseLocalParameterization) and td (a 1-vector), both in/out.
+ * Ceres' LM over 7 columns: Jacobi scaling, the LM diagonal, the damped Cholesky step and the model cost change over 7 columns,
+ * the parameter tolerance on the 8-vector (pose7, td), gradient_max_norm = max(|x - Plus(x, -g)|_inf over the pose, |g_td|).
+ * opt->fixed_mask bits 0-5 as in clc_solve_lm; bit 6 holds td at its start bits (bits 0-5 all set: only the offset is estimated,
+ * the extrinsic already known).  summary (may be NULL) and trace as clc_solve_lm's; device_ms covers the whole solve.  Also
+ * CLC_ERR_INVALID, checked first: a fixed_mask outside [0, 127), a trace_cap outside [0, 256] or > 0 without trace. */
+int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const clc_lm_options* opt, clc_lm_summary* summary,
+                             clc_lm_iteration* trace, int trace_cap);
+
 /* replaces: CamLaserCalClosedSolution(), reference src/LaseCamCalCeres.cpp:112-203.  Tlc16 row-major.
  * AtA81/Atb9 (the 9x9 normal equations) may be NULL. */
 int clc_closed_form(clc_problem* p, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
@@ -424,6 +467,9 @@ int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_of
 /* The same for one evaluation of clc_eval_poses on the path it picks: each bracket holds the K poses' frame constants, sweeps,
  * fix-up and reduction (or the one-cluster launch), not the copy to the host. */
 int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n, int flush_l2, float* ms_each);
+/* The same for one time-offset iteration at (pose7, td): each bracket holds the frames' planes and constants, the segment sweep,
+ * the fix-up into 36 sums per frame and the two-level reduction (clc_eval_time_offset without the copy to the host). */
+int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int n, int flush_l2, float* ms_each);
 /* The gather of clc_problem_subset(src, keep): `n` times a scratch subset is prepared, its gather kernel is timed alone (CUDA
  * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
  * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
