@@ -1177,41 +1177,50 @@ static int eval_all(clc_problem* const* ps, int n, const double pose7[7], int wh
   return first_rc;
 }
 
-static void unpack_H(const double* sums, double* H36) {
+extern "C++" {
+// The sums [upper-tri H | g | cost] of D tangent columns (clc::kLmSums) -> the full DxD H (row-major)
+template <int D>
+static void unpack_H(const double* sums, double* H) {
   int k = 0;
-  for (int i = 0; i < 6; ++i)
-    for (int j = i; j < 6; ++j) {
-      H36[i * 6 + j] = sums[k];
-      H36[j * 6 + i] = sums[k];
+  for (int i = 0; i < D; ++i)
+    for (int j = i; j < D; ++j) {
+      H[i * D + j] = sums[k];
+      H[j * D + i] = sums[k];
       ++k;
     }
 }
 
-static void eval_post(const double* sums, double H36[36], double g6[6], double* cost) {
-  if (H36) unpack_H(sums, H36);
-  if (g6) for (int i = 0; i < 6; ++i) g6[i] = sums[21 + i];
-  if (cost) *cost = sums[27];
+template <int D = 6>
+static void eval_post(const double* sums, double* H, double* g, double* cost) {
+  constexpr int kH = D * (D + 1) / 2;
+  if (H) unpack_H<D>(sums, H);
+  if (g) for (int i = 0; i < D; ++i) g[i] = sums[kH + i];
+  if (cost) *cost = sums[kH + D];
 }
 
-static void information_post(const double* sums, double H36[36], double b6[6], double* chi, double sv6[6], double V36[36]) {
-  double H[36];
-  unpack_H(sums, H);
-  if (H36) std::memcpy(H36, H, sizeof(H));
-  if (b6) for (int i = 0; i < 6; ++i) b6[i] = -sums[21 + i];
-  if (chi) *chi = 2.0 * sums[27];
-  if (sv6 || V36) {
+template <int D = 6>
+static void information_post(const double* sums, double* H_out, double* b, double* chi, double* sv, double* V_out) {
+  constexpr int kH = D * (D + 1) / 2;
+  double H[D * D];
+  unpack_H<D>(sums, H);
+  if (H_out) std::memcpy(H_out, H, sizeof(H));
+  if (b) for (int i = 0; i < D; ++i) b[i] = -sums[kH + i];
+  if (chi) *chi = 2.0 * sums[kH + D];
+  if (sv || V_out) {
     // H is symmetric: singular values = |eigenvalues|, right singular vectors = eigenvectors (Eigen::JacobiSVD, :366)
-    double w[6], V[36];
-    sym_eig<6>(H, w, V);
-    int order[6] = {0, 1, 2, 3, 4, 5};
-    std::sort(order, order + 6, [&](int a, int b) { return std::fabs(w[a]) > std::fabs(w[b]); });
-    for (int c = 0; c < 6; ++c) {
-      if (sv6) sv6[c] = std::fabs(w[order[c]]);
-      if (V36)
-        for (int r = 0; r < 6; ++r) V36[r * 6 + c] = V[r * 6 + order[c]];
+    double w[D], V[D * D];
+    sym_eig<D>(H, w, V);
+    int order[D];
+    for (int c = 0; c < D; ++c) order[c] = c;
+    std::sort(order, order + D, [&](int a, int c) { return std::fabs(w[a]) > std::fabs(w[c]); });
+    for (int c = 0; c < D; ++c) {
+      if (sv) sv[c] = std::fabs(w[order[c]]);
+      if (V_out)
+        for (int r = 0; r < D; ++r) V_out[r * D + c] = V[r * D + order[c]];
     }
   }
 }
+}  // extern "C++"
 
 static void closed_form_post(const double* sums, double Tlc[16], int* unobservable, double AtA81[81], double Atb9[9]) {
   double AtA[81], Atb[9];
@@ -1390,7 +1399,6 @@ namespace {
 
 struct SolveCtx {
   clc_lm_options opt;
-  int max_sweeps = 0;
   int launched = 0;
   bool fused_update = true, edges = false;
   int loss = clc::kLossCauchy;  // clc::LossKind
@@ -1430,6 +1438,74 @@ int l2_window(clc_problem* p, bool on) {
   return CLC_OK;
 }
 
+// every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps
+int lm_max_sweeps(const clc_lm_options& opt) { return opt.max_num_iterations + 2; }
+
+// The sweeps of the next batch between two host polls.  The first batch is twice as long: a solve from the identity or from the
+// closed form takes 6-16 sweeps (reference sizes and BASELINE configs alike), and every host poll in the middle of a solve stalls
+// the device for longer than the two or three no-op sweeps a too-long batch costs (a few microseconds each).
+int lm_batch(const clc_lm_options& opt, int launched, int max_sweeps) {
+  return std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
+}
+
+// The host loop of a batched on-device solve (segments, starts, time offset): enqueue() queues one LM iteration, in batches of
+// lm_batch, until lm_max_sweeps are queued or the device counter *d_running of solves still running reads 0 after a batch.  The
+// device time from the first iteration to the end of the last into *ms.
+int lm_batches(clc_problem* p, const clc_lm_options& opt, const int* d_running, const std::function<int()>& enqueue, float* ms) {
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+  const int max_sweeps = lm_max_sweeps(opt);
+  for (int launched = 0; launched < max_sweeps;) {
+    const int batch = lm_batch(opt, launched, max_sweeps);
+    for (int i = 0; i < batch; ++i) {
+      const int rc = enqueue();
+      if (rc != CLC_OK) return rc;
+    }
+    launched += batch;
+    CLC_CUDA(cudaMemcpyAsync(p->h_done, d_running, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(sync_stream_low_latency(p->stream));
+    if (*p->h_done == 0) break;  // no solve is running
+  }
+  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+  CLC_CUDA(cudaEventSynchronize(p->ev1));
+  CLC_CUDA(cudaEventElapsedTime(ms, p->ev0, p->ev1));
+  return CLC_OK;
+}
+
+extern "C++" {
+// The W states of a batched solve (to cores[W]) and their trace rows, trace_cap per solve, back on the host.
+template <int D>
+int lm_read_back(clc_problem* p, const clc::LmCoreN<D>* d_cores, int64_t W, const clc_lm_iteration* d_trace, int trace_cap,
+                 clc::LmCoreN<D>* cores, std::vector<clc_lm_iteration>* rows) {
+  rows->resize((size_t)W * trace_cap);
+  CLC_CUDA(cudaMemcpyAsync(cores, d_cores, sizeof(clc::LmCoreN<D>) * (size_t)W, cudaMemcpyDeviceToHost, p->stream));
+  if (trace_cap > 0)
+    CLC_CUDA(cudaMemcpyAsync(rows->data(), d_trace, sizeof(clc_lm_iteration) * rows->size(), cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  return CLC_OK;
+}
+
+template <int D>
+void summary_from_core(const clc::LmCoreN<D>& c, float ms, clc_lm_summary* sm) {
+  sm->termination = c.done ? c.done : CLC_TERM_NO_CONVERGENCE;
+  sm->num_iterations = c.n_trace;
+  sm->num_successful_steps = c.num_successful;
+  sm->num_unsuccessful_steps = c.num_unsuccessful;
+  sm->num_sweeps = c.sweeps;
+  sm->reserved = 0;
+  sm->initial_cost = c.initial_cost;
+  sm->final_cost = c.x_cost;
+  sm->device_ms = ms;
+}
+}  // extern "C++"
+
+// the rows a solve recorded (n_trace of them, at most kTraceMax were kept), up to the caller's trace_cap
+void copy_trace(const clc_lm_iteration* rows, int n_trace, int trace_cap, clc_lm_iteration* trace) {
+  const int n = std::min(std::min(n_trace, clc::kTraceMax), trace_cap);
+  for (int i = 0; i < n; ++i) trace[i] = rows[i];
+}
+
 int solve_begin(clc_problem* p, const double pose7[7], const clc_lm_options& opt, SolveCtx* ctx) {
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
@@ -1445,8 +1521,6 @@ int solve_begin(clc_problem* p, const double pose7[7], const clc_lm_options& opt
   ctx->fused_update = fused_lm_update(p);
   ctx->loss = p->loss_kind;
   ctx->edges = p->n_edges > 0;
-  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps
-  ctx->max_sweeps = opt.max_num_iterations + 2;
   ctx->launched = 0;
   *p->h_done = 0;
   return CLC_OK;
@@ -1506,39 +1580,27 @@ int solve_finish(clc_problem* p, double pose7[7], clc_lm_summary* summary, clc_l
   rc = check_p2p_error(p);
   if (rc != CLC_OK) return rc;
   const clc::LmCore& s = p->h_lm->core;
-  const clc_lm_iteration* dev_trace = p->h_lm->trace;
   if (pose7)
     for (int i = 0; i < 7; ++i) pose7[i] = s.x[i];  // the last accepted point (a terminating candidate is not applied)
-  if (summary) {
-    summary->termination = s.done ? s.done : CLC_TERM_NO_CONVERGENCE;
-    summary->num_iterations = s.n_trace;
-    summary->num_successful_steps = s.num_successful;
-    summary->num_unsuccessful_steps = s.num_unsuccessful;
-    summary->num_sweeps = s.sweeps;
-    summary->reserved = 0;
-    summary->initial_cost = s.initial_cost;
-    summary->final_cost = s.x_cost;
-    summary->device_ms = ms;
-  }
-  if (trace) {
-    const int n = std::min(std::min(s.n_trace, clc::kTraceMax), trace_cap);
-    for (int i = 0; i < n; ++i) trace[i] = dev_trace[i];
-  }
+  if (summary) summary_from_core(s, ms, summary);
+  if (trace) copy_trace(p->h_lm->trace, s.n_trace, trace_cap, trace);
   return CLC_OK;
 }
 
-// the first check of every LM entry point, before its other arguments and any device work
-int check_fixed_mask(const clc_lm_options* opt) {
-  if (opt && (opt->fixed_mask < 0 || opt->fixed_mask >= 63))
-    return fail(CLC_ERR_INVALID, "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)");
+// the first check of every LM entry point, before its other arguments and any device work (D: the solve's tangent columns, 6 or
+// 7 with the time offset)
+int check_fixed_mask(const clc_lm_options* opt, int D = 6) {
+  if (opt && (opt->fixed_mask < 0 || opt->fixed_mask >= (1 << D) - 1))
+    return fail(CLC_ERR_INVALID, D == 6 ? "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)"
+                                        : "fixed_mask must hold a proper subset of the seven coordinates (0 <= mask < 127)");
   return CLC_OK;
 }
 
 // the options of every LM entry point (NULL: defaults), checked before any device work
-int lm_options(const clc_lm_options* opt_in, clc_lm_options* opt) {
+int lm_options(const clc_lm_options* opt_in, clc_lm_options* opt, int D = 6) {
   if (opt_in) *opt = *opt_in; else clc_lm_default_options(opt);
   if (opt->max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
-  int rc = check_fixed_mask(opt);
+  int rc = check_fixed_mask(opt, D);
   if (rc != CLC_OK) return rc;
   if (opt->iterations_per_sync < 1) opt->iterations_per_sync = 1;
   return CLC_OK;
@@ -1563,7 +1625,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
         for (int g = 0; g < n; ++g) l2_demote(ps[g]);
     }
   } demote_on_exit{ps, n, true};
-  const int max_sweeps = ctx[0].max_sweeps;
+  const int max_sweeps = lm_max_sweeps(opt);
   int launched = 0;
   // Small problems (the reference's own sizes): the whole solve in one launch of one thread-block cluster that keeps every
   // residual in registers (clc_small.cuh) -- no TMA rings, no gather, no global round trip between two LM iterations.
@@ -1590,10 +1652,7 @@ int solve_all(clc_problem* const* ps, int n, double pose7[7], const clc_lm_optio
     launched = max_sweeps;
   }
   while (launched < max_sweeps) {
-    // the first batch is twice as long: a solve from the identity or from the closed form takes 6-16 sweeps (reference sizes and
-    // BASELINE configs alike), and every host poll in the middle of a solve stalls the device for longer than the two or three
-    // no-op sweeps a too-long batch costs (a few microseconds each)
-    const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
+    const int batch = lm_batch(opt, launched, max_sweeps);
     // iteration-major order: sweep i of every shard is queued before sweep i+1 of any, so no device's queue can fill up
     // with kernels that wait for a peer whose launches have not been issued yet
     for (int i = 0; i < batch; ++i)
@@ -1718,6 +1777,25 @@ int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, Segm
   return CLC_OK;
 }
 
+// Steps 4 and 5 of a segmented iteration over rows of kLmSums<D>: the reduction plan of r into sums ([W * kLmSums<D>]
+// or nullptr) and, with cores, lm_update on every segment that has not terminated (running, done: clc_segment_lm_kernel).
+extern "C++" template <int D>
+int segments_reduce(const SegmentRun& r, double* sums, clc::LmCoreN<D>* cores, clc_lm_iteration* trace, int trace_cap, int* running,
+                    int* done) {
+  clc_problem* p = r.p;
+  if (r.n_chunks > 0) {
+    const unsigned cb = (unsigned)((r.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+    clc::clc_segment_chunk_kernel<clc::kLmSums<D>><<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(
+        r.rows, r.chunk_offsets, r.n_chunks, done, r.partials);
+    CLC_LAUNCH_CHECK();
+  }
+  const unsigned sb = (unsigned)((r.W + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
+  clc::clc_segment_lm_kernel<D><<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.partials, r.seg_chunks, r.W, sums, cores, trace,
+                                                                                   trace_cap, running, done);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
 // One shared sweep of every segment: pose s at poses[s * pose_stride] on the device.  sums: [W * kNumSums] or nullptr; cores:
 // the solve's LmCores (lm_update runs on every segment that has not terminated), with its trace, counters and `done` flag.
 int segments_iteration(const SegmentRun& r, int loss, bool edges, const double* poses, int64_t pose_stride, double* sums,
@@ -1743,17 +1821,7 @@ int segments_iteration(const SegmentRun& r, int loss, bool edges, const double* 
     fixup<<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
     CLC_LAUNCH_CHECK();
   }
-  if (r.n_chunks > 0) {
-    const unsigned cb = (unsigned)((r.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-    clc::clc_segment_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.rows, r.chunk_offsets, r.n_chunks, done,
-                                                                                     r.partials);
-    CLC_LAUNCH_CHECK();
-  }
-  const unsigned sb = (unsigned)((r.W + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-  clc::clc_segment_lm_kernel<<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.partials, r.seg_chunks, r.W, sums, cores, trace,
-                                                                                trace_cap, counters, done);
-  CLC_LAUNCH_CHECK();
-  return CLC_OK;
+  return segments_reduce(r, sums, cores, trace, trace_cap, counters, done);
 }
 
 // the per-segment sums of one shared sweep at the poses [W * 7] (which: 0 eval, 1 information -- no loss, no edges)
@@ -1820,52 +1888,22 @@ int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg
   CLC_CUDA(cudaMemcpyAsync(r.cores, cores.data(), sizeof(clc::LmCore) * (size_t)W, cudaMemcpyHostToDevice, p->stream));
   const int counters0[2] = {(int)W, 0};
   CLC_CUDA(cudaMemcpyAsync(r.counters, counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
-  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
-  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
-  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
   const int loss = p->loss_kind;
   const bool edges = p->n_edges > 0;
   // the candidate pose of segment s: cores[s].cand, sizeof(LmCore) / 8 doubles apart
   const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.cores) + offsetof(clc::LmCore, cand));
   const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
-  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
-  const int max_sweeps = opt.max_num_iterations + 2;
-  int launched = 0;
-  while (launched < max_sweeps) {
-    // the first batch is twice as long, as in solve_all
-    const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
-    for (int i = 0; i < batch; ++i) {
-      rc = segments_iteration(r, loss, edges, cand, stride, nullptr, r.cores, r.trace, trace_cap, r.counters);
-      if (rc != CLC_OK) return rc;
-    }
-    launched += batch;
-    CLC_CUDA(cudaMemcpyAsync(p->h_done, r.counters, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-    CLC_CUDA(sync_stream_low_latency(p->stream));
-    if (*p->h_done == 0) break;  // no segment is running
-  }
-  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
-  CLC_CUDA(cudaMemcpyAsync(cores.data(), r.cores, sizeof(clc::LmCore) * (size_t)W, cudaMemcpyDeviceToHost, p->stream));
-  std::vector<clc_lm_iteration> rows((size_t)W * trace_cap);
-  if (trace_cap > 0)
-    CLC_CUDA(cudaMemcpyAsync(rows.data(), r.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
   float ms = 0.f;
-  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
+  std::vector<clc_lm_iteration> rows;
+  if ((rc = lm_batches(p, opt, r.counters, [&]() {
+         return segments_iteration(r, loss, edges, cand, stride, nullptr, r.cores, r.trace, trace_cap, r.counters);
+       }, &ms)) != CLC_OK ||
+      (rc = lm_read_back(p, r.cores, W, r.trace, trace_cap, cores.data(), &rows)) != CLC_OK)
+    return rc;
   for (int64_t s = 0; s < W; ++s) {
-    const clc::LmCore& c = cores[s];
-    for (int i = 0; i < 7; ++i) poses[7 * s + i] = c.x[i];  // the last accepted point, as clc_solve_lm
-    clc_lm_summary& sm = summaries[s];
-    sm.termination = c.done ? c.done : CLC_TERM_NO_CONVERGENCE;
-    sm.num_iterations = c.n_trace;
-    sm.num_successful_steps = c.num_successful;
-    sm.num_unsuccessful_steps = c.num_unsuccessful;
-    sm.num_sweeps = c.sweeps;
-    sm.reserved = 0;
-    sm.initial_cost = c.initial_cost;
-    sm.final_cost = c.x_cost;
-    sm.device_ms = ms;
-    const int n = std::min(c.n_trace, trace_cap);
-    for (int i = 0; i < n; ++i) trace[s * trace_cap + i] = rows[(size_t)s * trace_cap + i];
+    for (int i = 0; i < 7; ++i) poses[7 * s + i] = cores[s].x[i];  // the last accepted point, as clc_solve_lm
+    summary_from_core(cores[s], ms, &summaries[s]);
+    copy_trace(rows.data() + s * trace_cap, cores[s].n_trace, trace_cap, trace + s * trace_cap);
   }
   return CLC_OK;
 }
@@ -1897,8 +1935,8 @@ int check_time_offset(const clc_problem* p, const double* pose7, const double* t
 // evaluation, sums: its kTdSums sums), plus n, mdot, cdot of every frame and the solve's LM state.
 struct TimeRun {
   SegmentRun s;
-  double* tframe = nullptr;         // [n_frames * kTdFrameDoubles]
-  clc::LmCoreTd* core = nullptr;    // solve
+  double* tframe = nullptr;            // [n_frames * kTdFrameDoubles]
+  clc::LmCoreTd* core = nullptr;       // solve
   ~TimeRun() {
     if (!s.p) return;
     cudaSetDevice(s.p->device);
@@ -1916,11 +1954,12 @@ int time_prepare(clc_problem* p, TimeRun* r) {
   return CLC_OK;
 }
 
-// One iteration at pose8 = (pose7, td) on the device.  sums: [kTdSums] or nullptr; core: the solve's LM state (lm_update_td runs on
-// it), with its trace and `done` flag.
+// One iteration at pose8 = (pose7, td) on the device.  sums: [kTdSums] or nullptr; core: the solve's LM state (lm_update runs on
+// it), with its trace and counters (running, done) as segments_iteration's.
 int time_iteration(const TimeRun& r, int loss, const double* pose8, double* sums, clc::LmCoreTd* core, clc_lm_iteration* trace,
-                   int trace_cap, int* done) {
+                   int trace_cap, int* counters) {
   clc_problem* p = r.s.p;
+  int* done = counters != nullptr ? counters + 1 : nullptr;
   const clc::ProblemView v = make_view(p);
   const clc::TrajView tv = traj_view(p);
   const double* frame_time = p->traj + p->traj_knots;
@@ -1940,15 +1979,7 @@ int time_iteration(const TimeRun& r, int loss, const double* pose8, double* sums
     fixup<<<fb, threads, 0, p->stream>>>(v, r.s.consts, r.tframe, done, r.s.raw, r.s.slots, r.s.rows);
     CLC_LAUNCH_CHECK();
   }
-  if (r.s.n_chunks > 0) {
-    const unsigned cb = (unsigned)((r.s.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-    clc::clc_time_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.rows, r.s.chunk_offsets, r.s.n_chunks, done,
-                                                                                  r.s.partials);
-    CLC_LAUNCH_CHECK();
-  }
-  clc::clc_time_lm_kernel<<<1, 32, 0, p->stream>>>(r.s.partials, r.s.n_chunks, sums, core, trace, trace_cap, done);
-  CLC_LAUNCH_CHECK();
-  return CLC_OK;
+  return segments_reduce(r.s, sums, core, trace, trace_cap, counters, done);
 }
 
 // the point (pose7, td) and the sum buffers of an evaluation on the device
@@ -1976,11 +2007,6 @@ int time_eval_run(clc_problem* p, const double* pose7, double td, int which, dou
   CLC_CUDA(cudaMemcpyAsync(sums, r.s.sums, sizeof(double) * clc::kTdSums, cudaMemcpyDeviceToHost, p->stream));
   CLC_CUDA(cudaStreamSynchronize(p->stream));
   return CLC_OK;
-}
-
-void unpack_H7(const double* sums, double* H49) {
-  for (int i = 0; i < 7; ++i)
-    for (int j = i; j < 7; ++j) H49[i * 7 + j] = H49[j * 7 + i] = sums[clc::tri7(i, j)];
 }
 
 }  // namespace
@@ -2037,9 +2063,7 @@ int clc_eval_time_offset(clc_problem* p, const double pose7[7], double td, doubl
   double sums[clc::kTdSums];
   const int rc = time_eval_run(p, pose7, td, 0, sums);
   if (rc != CLC_OK) return rc;
-  if (H49) unpack_H7(sums, H49);
-  if (g7) for (int i = 0; i < 7; ++i) g7[i] = sums[28 + i];
-  if (cost) *cost = sums[35];
+  eval_post<7>(sums, H49, g7, cost);
   return CLC_OK;
 }
 
@@ -2048,90 +2072,43 @@ int clc_information_time_offset(clc_problem* p, const double pose7[7], double td
   double sums[clc::kTdSums];
   const int rc = time_eval_run(p, pose7, td, 1, sums);
   if (rc != CLC_OK) return rc;
-  double H[49];
-  unpack_H7(sums, H);
-  if (H49) std::memcpy(H49, H, sizeof(H));
-  if (b7) for (int i = 0; i < 7; ++i) b7[i] = -sums[28 + i];
-  if (chi) *chi = 2.0 * sums[35];
-  if (singular_values7 || V49) {
-    double w[7], V[49];
-    sym_eig<7>(H, w, V);
-    int order[7] = {0, 1, 2, 3, 4, 5, 6};
-    std::sort(order, order + 7, [&](int a, int b) { return std::fabs(w[a]) > std::fabs(w[b]); });
-    for (int c = 0; c < 7; ++c) {
-      if (singular_values7) singular_values7[c] = std::fabs(w[order[c]]);
-      if (V49)
-        for (int r = 0; r < 7; ++r) V49[r * 7 + c] = V[r * 7 + order[c]];
-    }
-  }
+  information_post<7>(sums, H49, b7, chi, singular_values7, V49);
   return CLC_OK;
 }
 
 int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const clc_lm_options* opt_in, clc_lm_summary* summary,
                              clc_lm_iteration* trace, int trace_cap) {
-  if (opt_in && (opt_in->fixed_mask < 0 || opt_in->fixed_mask >= 127))
-    return fail(CLC_ERR_INVALID, "fixed_mask must hold a proper subset of the seven coordinates (0 <= mask < 127)");
+  if (check_fixed_mask(opt_in, 7) != CLC_OK) return CLC_ERR_INVALID;
   if (trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
     return fail(CLC_ERR_INVALID, "trace_cap outside [0, 256], or without a trace array");
   int rc = check_time_offset(p, pose7, td);
   if (rc != CLC_OK) return rc;
   clc_lm_options opt;
-  if (opt_in) opt = *opt_in; else clc_lm_default_options(&opt);
-  if (opt.max_num_iterations < 0) return fail(CLC_ERR_INVALID, "max_num_iterations < 0");
-  if (opt.iterations_per_sync < 1) opt.iterations_per_sync = 1;
+  if ((rc = lm_options(opt_in, &opt, 7)) != CLC_OK) return rc;
   TimeRun r;
   if ((rc = time_prepare(p, &r)) != CLC_OK || (rc = seg_alloc(p, &r.core, 1)) != CLC_OK ||
-      (rc = seg_alloc(p, &r.s.counters, 1)) != CLC_OK)
+      (rc = seg_alloc(p, &r.s.counters, 2)) != CLC_OK)
     return rc;
   if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, trace_cap)) != CLC_OK) return rc;
   clc::LmCoreTd core;
   clc::lm_init_td(&core, pose7, *td, opt);
+  // pageable sources: each copy has read its source when it returns
   CLC_CUDA(cudaMemcpyAsync(r.core, &core, sizeof(core), cudaMemcpyHostToDevice, p->stream));
-  CLC_CUDA(cudaMemsetAsync(r.s.counters, 0, sizeof(int), p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));  // core is pageable and on this stack frame
-  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
-  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
-  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
+  const int counters0[2] = {1, 0};
+  CLC_CUDA(cudaMemcpyAsync(r.s.counters, counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
   const int loss = p->loss_kind;
   const double* cand = r.core->cand;  // (pose7, td) of the next sweep
-  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
-  const int max_sweeps = opt.max_num_iterations + 2;
-  int launched = 0;
-  while (launched < max_sweeps) {
-    // the first batch is twice as long, as in solve_all
-    const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
-    for (int i = 0; i < batch; ++i) {
-      rc = time_iteration(r, loss, cand, nullptr, r.core, r.s.trace, trace_cap, r.s.counters);
-      if (rc != CLC_OK) return rc;
-    }
-    launched += batch;
-    CLC_CUDA(cudaMemcpyAsync(p->h_done, r.s.counters, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-    CLC_CUDA(sync_stream_low_latency(p->stream));
-    if (*p->h_done != 0) break;
-  }
-  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
-  std::vector<clc_lm_iteration> rows((size_t)trace_cap);
-  CLC_CUDA(cudaMemcpyAsync(&core, r.core, sizeof(core), cudaMemcpyDeviceToHost, p->stream));
-  if (trace_cap > 0)
-    CLC_CUDA(cudaMemcpyAsync(rows.data(), r.s.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
   float ms = 0.f;
-  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
+  std::vector<clc_lm_iteration> rows;
+  if ((rc = lm_batches(p, opt, r.s.counters, [&]() {
+         return time_iteration(r, loss, cand, nullptr, r.core, r.s.trace, trace_cap, r.s.counters);
+       }, &ms)) != CLC_OK ||
+      (rc = lm_read_back(p, r.core, 1, r.s.trace, trace_cap, &core, &rows)) != CLC_OK)
+    return rc;
   for (int i = 0; i < 7; ++i) pose7[i] = core.x[i];  // the last accepted point, as clc_solve_lm
   *td = core.x[7];
-  if (summary) {
-    summary->termination = core.done ? core.done : CLC_TERM_NO_CONVERGENCE;
-    summary->num_iterations = core.n_trace;
-    summary->num_successful_steps = core.num_successful;
-    summary->num_unsuccessful_steps = core.num_unsuccessful;
-    summary->num_sweeps = core.sweeps;
-    summary->reserved = 0;
-    summary->initial_cost = core.initial_cost;
-    summary->final_cost = core.x_cost;
-    summary->device_ms = ms;
-  }
-  const int n = std::min(core.n_trace, trace_cap);
-  for (int i = 0; i < n; ++i) trace[i] = rows[(size_t)i];
+  if (summary) summary_from_core(core, ms, summary);
+  copy_trace(rows.data(), core.n_trace, trace_cap, trace);
   return CLC_OK;
 }
 
@@ -2237,17 +2214,8 @@ int poses_iteration(const PoseRun& r, int loss, bool edges, const double* poses,
                                          r.s.slots, slots_stride, r.s.rows);
     CLC_LAUNCH_CHECK();
   }
-  if (r.s.n_chunks > 0) {
-    const unsigned cb = (unsigned)((r.s.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-    clc::clc_segment_chunk_kernel<<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.rows, r.s.chunk_offsets, r.s.n_chunks, done,
-                                                                                     r.s.partials);
-    CLC_LAUNCH_CHECK();
-  }
-  const unsigned sb = (unsigned)((K + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-  clc::clc_segment_lm_kernel<<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.s.partials, r.s.seg_chunks, K, sums, cores, trace,
-                                                                                trace_cap, cores != nullptr ? r.running() : nullptr,
-                                                                                done);
-  CLC_LAUNCH_CHECK();
+  int rc = segments_reduce(r.s, sums, cores, trace, trace_cap, cores != nullptr ? r.running() : nullptr, done);
+  if (rc != CLC_OK) return rc;
   if (cores != nullptr) {
     clc::clc_pose_compact_kernel<<<1, clc::kPoseCompactThreads, 0, p->stream>>>(cores, (int)K, r.active, r.count());
     CLC_LAUNCH_CHECK();
@@ -2315,12 +2283,9 @@ int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const cl
   const int64_t K = n_poses;
   const int loss = p->loss_kind;
   const bool edges = p->n_edges > 0;
-  // every LM iteration needs exactly one sweep; invalid steps need none -> at most max_iterations + 1 sweeps (as solve_all)
-  const int max_sweeps = opt.max_num_iterations + 2;
   std::vector<clc::LmCore> cores((size_t)K);
   std::vector<clc_lm_iteration> rows;  // [K * trace_cap]
-  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
-  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  float ms = 0.f;
   if (p->loop_in_kernel >= 1 && fused_lm_update(p) && small_kernel_serves(p, edges)) {
     // the whole solve of every start in one launch, one cluster per start (the path clc_solve_lm takes for this problem)
     const SmallFn fn = small_poses_fn(loss, false);
@@ -2338,19 +2303,21 @@ int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const cl
     const size_t moved = trace_cap > 0 ? sizeof(clc::LmState) : sizeof(clc::LmCore);
     CLC_CUDA(cudaMemcpy2DAsync(d_states, sizeof(clc::LmState), states.data(), sizeof(clc::LmState), moved, (size_t)K,
                                cudaMemcpyHostToDevice, p->stream));
+    if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+    if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
     CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
-    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), d_states, max_sweeps, edges ? 1 : 0,
-                                                                                  nullptr, nullptr);
+    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), d_states, lm_max_sweeps(opt),
+                                                                                  edges ? 1 : 0, nullptr, nullptr);
     CLC_LAUNCH_CHECK();
     CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
     CLC_CUDA(cudaMemcpy2DAsync(states.data(), sizeof(clc::LmState), d_states, sizeof(clc::LmState), moved, (size_t)K,
                                cudaMemcpyDeviceToHost, p->stream));
     CLC_CUDA(cudaStreamSynchronize(p->stream));
+    CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
     rows.resize((size_t)K * trace_cap);
     for (int64_t k = 0; k < K; ++k) {
       cores[(size_t)k] = states[(size_t)k].core;
-      const int n = std::min(std::min(cores[(size_t)k].n_trace, clc::kTraceMax), trace_cap);
-      for (int i = 0; i < n; ++i) rows[(size_t)k * trace_cap + i] = states[(size_t)k].trace[i];
+      copy_trace(states[(size_t)k].trace, cores[(size_t)k].n_trace, trace_cap, rows.data() + k * trace_cap);
     }
   } else {
     PoseRun r;
@@ -2358,49 +2325,23 @@ int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const cl
     if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, (size_t)K * trace_cap)) != CLC_OK) return rc;
     for (int64_t k = 0; k < K; ++k) clc::lm_init(&cores[(size_t)k], poses + 7 * k, opt);
     CLC_CUDA(cudaMemcpyAsync(r.s.cores, cores.data(), sizeof(clc::LmCore) * (size_t)K, cudaMemcpyHostToDevice, p->stream));
-    CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
     // the candidate pose of start k: cores[k].cand, sizeof(LmCore) / 8 doubles apart
     const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.s.cores) + offsetof(clc::LmCore, cand));
     const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
-    int launched = 0;
-    while (launched < max_sweeps) {
-      // the first batch is twice as long, as in solve_all
-      const int batch = std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
-      for (int i = 0; i < batch; ++i)
-        if ((rc = poses_iteration(r, loss, edges, cand, stride, nullptr, r.s.cores, r.s.trace, trace_cap)) != CLC_OK) return rc;
-      launched += batch;
-      CLC_CUDA(cudaMemcpyAsync(p->h_done, r.running(), sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-      CLC_CUDA(sync_stream_low_latency(p->stream));
-      if (*p->h_done == 0) break;  // no start is running
-    }
-    CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
-    CLC_CUDA(cudaMemcpyAsync(cores.data(), r.s.cores, sizeof(clc::LmCore) * (size_t)K, cudaMemcpyDeviceToHost, p->stream));
-    rows.resize((size_t)K * trace_cap);
-    if (trace_cap > 0)
-      CLC_CUDA(cudaMemcpyAsync(rows.data(), r.s.trace, sizeof(clc_lm_iteration) * rows.size(), cudaMemcpyDeviceToHost, p->stream));
-    CLC_CUDA(cudaStreamSynchronize(p->stream));
+    if ((rc = lm_batches(p, opt, r.running(), [&]() {
+           return poses_iteration(r, loss, edges, cand, stride, nullptr, r.s.cores, r.s.trace, trace_cap);
+         }, &ms)) != CLC_OK ||
+        (rc = lm_read_back(p, r.s.cores, K, r.s.trace, trace_cap, cores.data(), &rows)) != CLC_OK)
+      return rc;
   }
-  float ms = 0.f;
-  CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
   std::vector<int> term((size_t)K);
   std::vector<double> final_cost((size_t)K);
   for (int64_t k = 0; k < K; ++k) {
-    const clc::LmCore& c = cores[(size_t)k];
-    for (int i = 0; i < 7; ++i) poses[7 * k + i] = c.x[i];  // the last accepted point, as clc_solve_lm
-    clc_lm_summary& sm = summaries[k];
-    sm.termination = c.done ? c.done : CLC_TERM_NO_CONVERGENCE;
-    sm.num_iterations = c.n_trace;
-    sm.num_successful_steps = c.num_successful;
-    sm.num_unsuccessful_steps = c.num_unsuccessful;
-    sm.num_sweeps = c.sweeps;
-    sm.reserved = 0;
-    sm.initial_cost = c.initial_cost;
-    sm.final_cost = c.x_cost;
-    sm.device_ms = ms;
-    term[(size_t)k] = sm.termination;
-    final_cost[(size_t)k] = sm.final_cost;
-    const int n = std::min(c.n_trace, trace_cap);
-    for (int i = 0; i < n; ++i) trace[k * trace_cap + i] = rows[(size_t)k * trace_cap + i];
+    for (int i = 0; i < 7; ++i) poses[7 * k + i] = cores[(size_t)k].x[i];  // the last accepted point, as clc_solve_lm
+    summary_from_core(cores[(size_t)k], ms, &summaries[k]);
+    term[(size_t)k] = summaries[k].termination;
+    final_cost[(size_t)k] = summaries[k].final_cost;
+    copy_trace(rows.data() + k * trace_cap, cores[(size_t)k].n_trace, trace_cap, trace + k * trace_cap);
   }
   if (best) *best = clc::best_start(K, term.data(), final_cost.data(), CLC_TERM_FAILURE);
   return CLC_OK;

@@ -18,11 +18,17 @@
 namespace clc {
 
 constexpr int kTraceMax = 256;
-constexpr int kNumSums = 28;  // 21 upper-tri H + 6 g + 1 cost
+
+// The state machine runs over D tangent columns: D = 6, the pose (its local parameterization), or D = 7, the pose and the
+// camera-laser time offset td as a plain 1-vector (clc_time_offset.cuh).  Its sums are [upper-tri H | g | cost].
+template <int D>
+constexpr int kLmSums = D * (D + 1) / 2 + D + 1;
+constexpr int kNumSums = kLmSums<6>;  // 21 upper-tri H + 6 g + 1 cost
 
 // Hot state of the minimiser (about 600 bytes): staged through shared memory around lm_update so that the single
 // thread running it does not pay a global-memory round trip per field.
-struct LmCore {
+template <int D>
+struct LmCoreN {
   int done;            // CLC_TERM_*; 0 while running
   int phase;           // 0: the pending sweep evaluates the start point; 1: it evaluates a candidate
   int iteration;       // index of the last finalised iteration
@@ -33,17 +39,20 @@ struct LmCore {
   int num_unsuccessful;
   int sweeps;
   int pad0;
-  double x[7];
-  double cand[7];      // the pose the next sweep evaluates
+  double x[D + 1];     // pose7 (D = 7: then td)
+  double cand[D + 1];  // the point the next sweep evaluates
   double x_cost, x_norm;
-  double H[21], g[6];  // at x: loss-corrected, unscaled
-  double scale[6], diag[6];
+  double H[D * (D + 1) / 2], g[D];  // at x: loss-corrected, unscaled
+  double scale[D], diag[D];
   double radius, decrease_factor, model_cost_change;
   double initial_cost;
   clc_lm_options opt;
 };
-static_assert(sizeof(LmCore) % 8 == 0, "LmCore is copied as 8-byte words");
-constexpr int kLmCoreWords = (int)(sizeof(LmCore) / 8);
+using LmCore = LmCoreN<6>;
+static_assert(sizeof(LmCore) % 8 == 0 && sizeof(LmCoreN<7>) % 8 == 0, "LmCoreN is copied as 8-byte words");
+template <int D>
+constexpr int kLmWords = (int)(sizeof(LmCoreN<D>) / 8);
+constexpr int kLmCoreWords = kLmWords<6>;
 
 struct LmState {
   LmCore core;
@@ -61,13 +70,15 @@ __device__ long long g_lm_profile[16];
 #define CLC_LM_STAMP(i) ((void)0)
 #endif
 
-CLC_HD double norm7(const double* a) {
+template <int N>
+CLC_HD double vec_norm(const double* a) {
   double s = 0.0;
-  for (int i = 0; i < 7; ++i) s += a[i] * a[i];
+  for (int i = 0; i < N; ++i) s += a[i] * a[i];
   return sqrt(s);
 }
 
-// Ceres EvaluateGradientAndJacobian: |x - Plus(x, -g)|_inf
+// Ceres EvaluateGradientAndJacobian: |x - Plus(x, -g)|_inf, over the pose and (D = 7) td
+template <int D>
 CLC_HD double gradient_max_norm(const double* x, const double* g) {
   double ng[6], xp[7], m = 0.0;
   for (int i = 0; i < 6; ++i) ng[i] = -g[i];
@@ -75,6 +86,10 @@ CLC_HD double gradient_max_norm(const double* x, const double* g) {
   for (int i = 0; i < 7; ++i) {
     const double d = fabs(x[i] - xp[i]);
     if (d > m) m = d;
+  }
+  if constexpr (D == 7) {
+    const double a = fabs(g[6]);
+    if (a > m) m = a;
   }
   return m;
 }
@@ -84,26 +99,31 @@ CLC_HD double gradient_max_norm(const double* x, const double* g) {
 // then sees the free coordinates only -- gradient_max_norm (g embedded with zeros), the Jacobi-scaled system and its LM
 // diagonal, whose positive pivot makes the Cholesky step of a held coordinate exactly 0 and that of the free ones the step of
 // the reduced system (every product with a held entry is 0), and the model cost change.  Done in place on the state (shared
-// memory on the device), off the register-resident step code.
-CLC_HD void lm_hold(LmCore* s, int fixed) {
+// memory on the device), off the register-resident step code.  With D = 7, bit 6 holds td.
+template <int D>
+CLC_HD void lm_hold(LmCoreN<D>* s, int fixed) {
 #pragma unroll 1
-  for (int k = 0; k < 6; ++k) {
+  for (int k = 0; k < D; ++k) {
     if (!(fixed >> k & 1)) continue;
 #pragma unroll 1
-    for (int j = 0; j < 6; ++j) s->H[j < k ? tri(j, k) : tri(k, j)] = 0.0;
-    s->H[tri(k, k)] = 1.0;
+    for (int j = 0; j < D; ++j) s->H[j < k ? tri<D>(j, k) : tri<D>(k, j)] = 0.0;
+    s->H[tri<D>(k, k)] = 1.0;
     s->g[k] = 0.0;
   }
 }
 
-// a held translation of the candidate keeps the bits of x (x + 0 would turn a -0.0 into +0.0)
-CLC_HD void lm_hold_cand(LmCore* s, int fixed) {
+// a held translation of the candidate (or td) keeps the bits of x (x + 0 would turn a -0.0 into +0.0)
+template <int D>
+CLC_HD void lm_hold_cand(LmCoreN<D>* s, int fixed) {
 #pragma unroll 1
   for (int k = 0; k < 3; ++k)
     if (fixed >> k & 1) s->cand[k] = s->x[k];
+  if constexpr (D == 7)
+    if (fixed >> 6 & 1) s->cand[7] = s->x[7];
 }
 
-CLC_HD void lm_record(LmCore* s, clc_lm_iteration* trace, const clc_lm_iteration& it) {
+template <int D>
+CLC_HD void lm_record(LmCoreN<D>* s, clc_lm_iteration* trace, const clc_lm_iteration& it) {
   if (s->n_trace < kTraceMax) trace[s->n_trace] = it;
   s->n_trace++;
 }
@@ -115,17 +135,20 @@ struct TraceRows {
   int cap;
 };
 
-CLC_HD void lm_record(LmCore* s, TraceRows trace, const clc_lm_iteration& it) {
+template <int D>
+CLC_HD void lm_record(LmCoreN<D>* s, TraceRows trace, const clc_lm_iteration& it) {
   if (s->n_trace < trace.cap) trace.rows[s->n_trace] = it;
   s->n_trace++;
 }
 
-CLC_HD void lm_init(LmCore* s, const double* pose7, const clc_lm_options& opt) {
+// x0: pose7 (D = 7: then td)
+template <int D>
+CLC_HD void lm_init(LmCoreN<D>* s, const double* x0, const clc_lm_options& opt) {
   s->done = 0; s->phase = 0; s->iteration = 0; s->num_invalid = 0; s->reuse_diagonal = 0; s->n_trace = 0;
   s->num_successful = 0; s->num_unsuccessful = 0; s->sweeps = 0; s->pad0 = 0;
-  for (int i = 0; i < 7; ++i) { s->x[i] = pose7[i]; s->cand[i] = pose7[i]; }
+  for (int i = 0; i < D + 1; ++i) { s->x[i] = x0[i]; s->cand[i] = x0[i]; }
   s->x_cost = 0.0;
-  s->x_norm = norm7(pose7);
+  s->x_norm = vec_norm<D + 1>(x0);
   s->radius = opt.initial_trust_region_radius;
   s->decrease_factor = 2.0;
   s->model_cost_change = 0.0;
@@ -133,11 +156,13 @@ CLC_HD void lm_init(LmCore* s, const double* pose7, const clc_lm_options& opt) {
   s->opt = opt;
 }
 
-// Consumes the 28 sums of the sweep that has just evaluated s->cand and advances the minimiser until it either
+// Consumes the kLmSums<D> sums of the sweep that has just evaluated s->cand and advances the minimiser until it either
 // terminates (s->done != 0) or has a new candidate in s->cand for the next sweep.  Trace: a clc_lm_iteration* of kTraceMax
-// rows, or TraceRows.
-template <class Trace>
-CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
+// rows, or TraceRows.  With D = 7 the parameter tolerance measures the 8-vector (pose7, td), gradient_max_norm also takes |g_td|
+// and the candidate's td is x_td + its step.
+template <int D, class Trace>
+CLC_HD void lm_update(LmCoreN<D>* s, Trace trace, const double* sums) {
+  constexpr int kH = D * (D + 1) / 2, kSums = kLmSums<D>;
   if (s->done) return;
   CLC_LM_STAMP(0);
   s->sweeps++;
@@ -147,26 +172,26 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
   // Ceres rejects an evaluation that produced a non-finite residual or Jacobian entry (residual_block.cc
   // IsArrayValid): at the start point that is a FAILURE, at a candidate it is "a step with infinite cost".
   bool sums_ok = true;
-  for (int i = 0; i < kNumSums; ++i) sums_ok = sums_ok && is_finite(sums[i]);
+  for (int i = 0; i < kSums; ++i) sums_ok = sums_ok && is_finite(sums[i]);
   if (s->phase == 0) {
     // ---- iteration 0 (Ceres: IterationZero) ----
     if (!sums_ok) { s->done = CLC_TERM_FAILURE; return; }
-    s->x_cost = sums[27];
-    for (int i = 0; i < 21; ++i) s->H[i] = sums[i];
-    for (int i = 0; i < 6; ++i) s->g[i] = sums[21 + i];
+    s->x_cost = sums[kSums - 1];
+    for (int i = 0; i < kH; ++i) s->H[i] = sums[i];
+    for (int i = 0; i < D; ++i) s->g[i] = sums[kH + i];
     if (o.fixed_mask) lm_hold(s, o.fixed_mask);
-    for (int k = 0; k < 6; ++k) s->scale[k] = o.jacobi_scaling ? 1.0 / (1.0 + sqrt(s->H[tri(k, k)])) : 1.0;
+    for (int k = 0; k < D; ++k) s->scale[k] = o.jacobi_scaling ? 1.0 / (1.0 + sqrt(s->H[tri<D>(k, k)])) : 1.0;
     s->initial_cost = s->x_cost;
     last.iteration = 0; last.step_is_valid = 1; last.step_is_successful = 1;
-    last.cost = s->x_cost; last.cost_change = 0.0; last.gradient_max_norm = gradient_max_norm(s->x, s->g);
+    last.cost = s->x_cost; last.cost_change = 0.0; last.gradient_max_norm = gradient_max_norm<D>(s->x, s->g);
     last.step_norm = 0.0; last.relative_decrease = 0.0; last.trust_region_radius = s->radius;
   } else {
     // ---- a candidate has been evaluated ----
-    const double cand_cost = sums_ok ? sums[27] : DBL_MAX;
+    const double cand_cost = sums_ok ? sums[kSums - 1] : DBL_MAX;
     last.iteration = s->iteration + 1; last.step_is_valid = 1; last.step_is_successful = 0;
-    double d[7];
-    for (int i = 0; i < 7; ++i) d[i] = s->x[i] - s->cand[i];
-    last.step_norm = norm7(d);
+    double d[D + 1];
+    for (int i = 0; i < D + 1; ++i) d[i] = s->x[i] - s->cand[i];
+    last.step_norm = vec_norm<D + 1>(d);
     last.cost_change = s->x_cost - cand_cost;
     last.cost = cand_cost;
     last.gradient_max_norm = 0.0; last.relative_decrease = 0.0; last.trust_region_radius = s->radius;
@@ -185,14 +210,14 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
     last.relative_decrease = last.cost_change / s->model_cost_change;
     if (last.relative_decrease > o.min_relative_decrease) {
       // Ceres: HandleSuccessfulStep + LevenbergMarquardtStrategy::StepAccepted
-      for (int i = 0; i < 7; ++i) s->x[i] = s->cand[i];
-      s->x_norm = norm7(s->x);
+      for (int i = 0; i < D + 1; ++i) s->x[i] = s->cand[i];
+      s->x_norm = vec_norm<D + 1>(s->x);
       s->x_cost = cand_cost;
-      for (int i = 0; i < 21; ++i) s->H[i] = sums[i];
-      for (int i = 0; i < 6; ++i) s->g[i] = sums[21 + i];
+      for (int i = 0; i < kH; ++i) s->H[i] = sums[i];
+      for (int i = 0; i < D; ++i) s->g[i] = sums[kH + i];
       if (o.fixed_mask) lm_hold(s, o.fixed_mask);
       last.step_is_successful = 1;
-      last.gradient_max_norm = gradient_max_norm(s->x, s->g);
+      last.gradient_max_norm = gradient_max_norm<D>(s->x, s->g);
       const double q = 2.0 * last.relative_decrease - 1.0;
       double den = 1.0 - q * q * q;
       if (den < 1.0 / 3.0) den = 1.0 / 3.0;
@@ -224,36 +249,36 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
 
     CLC_LM_STAMP(2);  // iteration recorded, termination tests done
     // ---- Ceres: LevenbergMarquardtStrategy::ComputeStep on the Jacobi-scaled system ----
-    double Hs[36], gs[6], A[36], step[6];
+    double Hs[D * D], gs[D], A[D * D], step[D];
 #pragma unroll
-    for (int i = 0; i < 6; ++i) {
+    for (int i = 0; i < D; ++i) {
       gs[i] = s->scale[i] * s->g[i];
 #pragma unroll
-      for (int j = i; j < 6; ++j) {
-        const double v = s->scale[i] * s->scale[j] * s->H[tri(i, j)];
-        Hs[i * 6 + j] = v;
-        Hs[j * 6 + i] = v;
+      for (int j = i; j < D; ++j) {
+        const double v = s->scale[i] * s->scale[j] * s->H[tri<D>(i, j)];
+        Hs[i * D + j] = v;
+        Hs[j * D + i] = v;
       }
     }
     if (!s->reuse_diagonal)
 #pragma unroll
-      for (int k = 0; k < 6; ++k) {
-        double dd = Hs[k * 6 + k];
+      for (int k = 0; k < D; ++k) {
+        double dd = Hs[k * D + k];
         dd = dd > o.min_lm_diagonal ? dd : o.min_lm_diagonal;
         dd = dd < o.max_lm_diagonal ? dd : o.max_lm_diagonal;
         s->diag[k] = dd;
       }
 #pragma unroll
-    for (int i = 0; i < 36; ++i) A[i] = Hs[i];
+    for (int i = 0; i < D * D; ++i) A[i] = Hs[i];
     const double inv_radius = 1.0 / s->radius;
 #pragma unroll
-    for (int k = 0; k < 6; ++k) A[k * 6 + k] += s->diag[k] * inv_radius;  // D^2 = diag / radius
+    for (int k = 0; k < D; ++k) A[k * D + k] += s->diag[k] * inv_radius;  // D^2 = diag / radius
     CLC_LM_STAMP(3);  // scaled, damped system built
-    bool ok = chol6_solve(A, gs, step);
+    bool ok = chol_solve<D>(A, gs, step);
     CLC_LM_STAMP(4);  // Cholesky solve done
     s->reuse_diagonal = 1;
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
+    for (int k = 0; k < D; ++k) {
       if (!is_finite(step[k])) ok = false;
       step[k] = -step[k];
     }
@@ -262,11 +287,11 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
     if (ok) {
       double gs_s = 0.0, sHs = 0.0;
 #pragma unroll
-      for (int i = 0; i < 6; ++i) {
+      for (int i = 0; i < D; ++i) {
         gs_s += gs[i] * step[i];
         double r = 0.0;
 #pragma unroll
-        for (int j = 0; j < 6; ++j) r += Hs[i * 6 + j] * step[j];
+        for (int j = 0; j < D; ++j) r += Hs[i * D + j] * step[j];
         sHs += step[i] * r;
       }
       mcc = -gs_s - 0.5 * sHs;
@@ -284,10 +309,11 @@ CLC_HD void lm_update(LmCore* s, Trace trace, const double* sums) {
       continue;
     }
     s->num_invalid = 0;
-    double delta[6];
-    for (int k = 0; k < 6; ++k) delta[k] = step[k] * s->scale[k];
+    double delta[D];
+    for (int k = 0; k < D; ++k) delta[k] = step[k] * s->scale[k];
     CLC_LM_STAMP(5);  // model cost change done
     pose_plus(s->x, delta, s->cand);
+    if constexpr (D == 7) s->cand[7] = s->x[7] + delta[6];
     if (o.fixed_mask) lm_hold_cand(s, o.fixed_mask);
     s->model_cost_change = mcc;
     s->phase = 1;

@@ -251,50 +251,54 @@ CLC_HD double gen_noise(uint64_t seed, double sigma, int64_t frame, int64_t beam
   return sigma * sqrt(-2.0 * log(1.0 - u1)) * cos(2.0 * kPi * u2);
 }
 
-// ---- 6x6 dense pieces of the LM step ------------------------------------------------------------------------
+// ---- dense pieces of the LM step (6 columns: the pose; 7: the pose and the time offset) ------------------------------
 
-CLC_HD int tri(int i, int j) { return i * 6 - (i * (i - 1)) / 2 + (j - i); }  // upper-tri index, i <= j
+template <int N = 6>
+CLC_HD int tri(int i, int j) { return i * N - (i * (i - 1)) / 2 + (j - i); }  // upper-tri index of the NxN, i <= j
 
-// Cholesky solve of the SPD 6x6 system A y = b (A full row-major).  false if not positive definite.
-CLC_HD bool chol6_solve(const double* A, const double* b, double* y) {
+// Cholesky solve of the SPD NxN system A y = b (A full row-major).  false if not positive definite.
+template <int N>
+CLC_HD bool chol_solve(const double* A, const double* b, double* y) {
   // fully unrolled (L, z, inv live in registers): it always runs on the same SM (block 0), whose instruction cache keeps it.
   // One reciprocal per pivot instead of one division per entry (divisions are ~100-cycle subroutines in FP64).
-  double L[36], inv[6];
+  double L[N * N], inv[N];
   bool ok = true;
 #pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    double s = A[j * 6 + j];
+  for (int j = 0; j < N; ++j) {
+    double s = A[j * N + j];
 #pragma unroll
-    for (int k = 0; k < j; ++k) s -= L[j * 6 + k] * L[j * 6 + k];
+    for (int k = 0; k < j; ++k) s -= L[j * N + k] * L[j * N + k];
     ok = ok && (s > 0.0);
     const double d = sqrt(s);
-    L[j * 6 + j] = d;
+    L[j * N + j] = d;
     inv[j] = 1.0 / d;
 #pragma unroll
-    for (int i = j + 1; i < 6; ++i) {
-      double t = A[i * 6 + j];
+    for (int i = j + 1; i < N; ++i) {
+      double t = A[i * N + j];
 #pragma unroll
-      for (int k = 0; k < j; ++k) t -= L[i * 6 + k] * L[j * 6 + k];
-      L[i * 6 + j] = t * inv[j];
+      for (int k = 0; k < j; ++k) t -= L[i * N + k] * L[j * N + k];
+      L[i * N + j] = t * inv[j];
     }
   }
   if (!ok) return false;
-  double z[6];
+  double z[N];
 #pragma unroll
-  for (int i = 0; i < 6; ++i) {
+  for (int i = 0; i < N; ++i) {
     double s = b[i];
 #pragma unroll
-    for (int k = 0; k < i; ++k) s -= L[i * 6 + k] * z[k];
+    for (int k = 0; k < i; ++k) s -= L[i * N + k] * z[k];
     z[i] = s * inv[i];
   }
 #pragma unroll
-  for (int i = 5; i >= 0; --i) {
+  for (int i = N - 1; i >= 0; --i) {
     double s = z[i];
 #pragma unroll
-    for (int k = i + 1; k < 6; ++k) s -= L[k * 6 + i] * y[k];
+    for (int k = i + 1; k < N; ++k) s -= L[k * N + i] * y[k];
     y[i] = s * inv[i];
   }
   return true;
 }
+
+CLC_HD bool chol6_solve(const double* A, const double* b, double* y) { return chol_solve<6>(A, b, y); }
 
 }  // namespace clc

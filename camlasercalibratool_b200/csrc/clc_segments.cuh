@@ -9,6 +9,8 @@
 //   3. clc_segment_fixup_kernel    every frame's share of the 28 sums at its segment's pose (zeros for an empty frame);
 //   4. clc_segment_chunk_kernel    level 1 of the fixed reduction plan (clc_segment_plan.h): the rows of every chunk;
 //   5. clc_segment_lm_kernel       level 2: the chunk partials of every segment, then lm_update on the segment's own LmCore.
+// Steps 4 and 5 are templates on the row width and the number of tangent columns: the time offset (clc_time_offset.cuh) runs
+// them as one segment of 36-wide rows and a 7-column LmCoreN<7>.
 // Every kernel of the iteration is a no-op once every segment has terminated (`done`, raised by the last one).
 // The kernels at the end of the file run the same iteration for one calibration at many poses.
 #pragma once
@@ -126,50 +128,62 @@ __global__ void clc_segment_fixup_kernel(ProblemView pv, const double* __restric
   segment_fixup_frame<LOSS>(pv, consts, edges, f, raw, slots, rows);
 }
 
-// Level 1: one warp per chunk, lane k < kNumSums adds output k of the chunk's rows in frame order.
+// Level 1: one warp per chunk, lane k adds outputs k, k + 32, ... (< W) of the chunk's W-wide rows in frame order.
 constexpr int kSegWarpsPerBlock = 4;
+template <int W>
 __global__ void __launch_bounds__(32 * kSegWarpsPerBlock)
 clc_segment_chunk_kernel(const double* __restrict__ rows, const int64_t* __restrict__ chunk_offsets, int64_t n_chunks,
                          const int* done, double* __restrict__ partials) {
   const int64_t ch = (int64_t)blockIdx.x * kSegWarpsPerBlock + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  if (ch >= n_chunks || lane >= kNumSums || (done != nullptr && *done != 0)) return;
+  if (ch >= n_chunks || lane >= W || (done != nullptr && *done != 0)) return;
   const int64_t a = chunk_offsets[ch], b = chunk_offsets[ch + 1];
-  double acc = 0.0;
-  for (int64_t r = a; r < b; ++r) acc += rows[r * kNumSums + lane];
-  partials[ch * kNumSums + lane] = acc;
+#pragma unroll
+  for (int j = 0; j < (W + 31) / 32; ++j) {
+    const int k = lane + 32 * j;
+    if (k >= W) break;
+    double acc = 0.0;
+    for (int64_t r = a; r < b; ++r) acc += rows[r * W + k];
+    partials[ch * W + k] = acc;
+  }
 }
 
-// Level 2 + LM: one warp per segment.  Lane k < kNumSums adds output k of the segment's chunk partials in chunk order (an empty
-// segment sums to zeros) into sums[s] (may be nullptr); with cores, lane 0 then runs lm_update on segment s's LmCore, staged in
-// shared memory.  A segment that terminates in this call leaves `running`; the last one raises `done`.
+// Level 2 + LM over D tangent columns: one warp per segment.  Lane k adds outputs k, k + 32, ... (< kLmSums<D>) of the
+// segment's chunk partials in chunk order (an empty segment sums to zeros) into sums[s] (may be nullptr); with cores, lane 0 then
+// runs lm_update on segment s's LmCoreN<D>, staged in shared memory.  A segment that terminates in this call leaves `running`; the
+// last one raises `done`.
+template <int D>
 __global__ void __launch_bounds__(32 * kSegWarpsPerBlock)
 clc_segment_lm_kernel(const double* __restrict__ partials, const int64_t* __restrict__ seg_chunks, int64_t n_segments,
-                      double* sums, LmCore* cores, clc_lm_iteration* trace, int trace_cap, int* running, int* done) {
-  __shared__ unsigned long long s_core[kSegWarpsPerBlock][kLmCoreWords];
-  __shared__ double s_sums[kSegWarpsPerBlock][32];
+                      double* sums, LmCoreN<D>* cores, clc_lm_iteration* trace, int trace_cap, int* running, int* done) {
+  constexpr int W = kLmSums<D>, kWords = kLmWords<D>;
+  __shared__ unsigned long long s_core[kSegWarpsPerBlock][kWords];
+  __shared__ double s_sums[kSegWarpsPerBlock][(W + 31) / 32 * 32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t s = (int64_t)blockIdx.x * kSegWarpsPerBlock + warp;
   if (s >= n_segments || (done != nullptr && *done != 0)) return;
   const int64_t c0 = seg_chunks[s], c1 = seg_chunks[s + 1];
-  if (lane < kNumSums) {
+#pragma unroll
+  for (int j = 0; j < (W + 31) / 32; ++j) {
+    const int k = lane + 32 * j;
+    if (k >= W) break;
     double acc = 0.0;
-    for (int64_t c = c0; c < c1; ++c) acc += partials[c * kNumSums + lane];
-    s_sums[warp][lane] = acc;
-    if (sums != nullptr) sums[s * kNumSums + lane] = acc;
+    for (int64_t c = c0; c < c1; ++c) acc += partials[c * W + k];
+    s_sums[warp][k] = acc;
+    if (sums != nullptr) sums[s * W + k] = acc;
   }
   if (cores == nullptr) return;
   unsigned long long* g_core = reinterpret_cast<unsigned long long*>(cores + s);
-  for (int k = lane; k < kLmCoreWords; k += 32) s_core[warp][k] = g_core[k];
+  for (int k = lane; k < kWords; k += 32) s_core[warp][k] = g_core[k];
   __syncwarp();
   if (lane == 0) {
-    LmCore* core = reinterpret_cast<LmCore*>(s_core[warp]);
+    LmCoreN<D>* core = reinterpret_cast<LmCoreN<D>*>(s_core[warp]);
     const bool was_running = core->done == 0;
     lm_update(core, TraceRows{trace != nullptr ? trace + s * trace_cap : nullptr, trace_cap}, s_sums[warp]);
     if (was_running && core->done != 0 && atomicSub(running, 1) == 1) *done = 1;
   }
   __syncwarp();
-  for (int k = lane; k < kLmCoreWords; k += 32) g_core[k] = s_core[warp][k];
+  for (int k = lane; k < kWords; k += 32) g_core[k] = s_core[warp][k];
 }
 
 

@@ -15,8 +15,8 @@
 //                               n, mdot, cdot into a per-frame array;
 //   2. clc_sweep_kernel<.., kModeSegments, ..>   unchanged;
 //   3. clc_time_fixup_kernel    every frame's moments (segment_frame_moments) expanded into its row of kTdSums;
-//   4. clc_time_chunk_kernel    level 1 of the segment plan at width kTdSums;
-//   5. clc_time_lm_kernel       level 2, then lm_update_td (Ceres' LM on the pose and td) by lane 0.
+//   4. clc_segment_chunk_kernel<kTdSums>   level 1 of the segment plan;
+//   5. clc_segment_lm_kernel<7>            level 2, then lm_update on LmCoreN<7> (Ceres' LM on the pose and td, clc_lm.cuh).
 // The host part (everything CLC_HD) also compiles with g++ for the CPU tests.
 #pragma once
 
@@ -25,11 +25,9 @@
 
 namespace clc {
 
-constexpr int kTdSums = 36;          // 28 upper-tri of the 7x7 H (tx ty tz rx ry rz td, row-major, i <= j) + 7 g + 1 cost
-constexpr int kTdFrameDoubles = 8;   // per frame: n[3], mdot[3], cdot, unused
-constexpr int kKnotDoubles = 7;      // per knot: q_ac (x, y, z, w), t_ac
-
-CLC_HD int tri7(int i, int j) { return i * 7 - (i * (i - 1)) / 2 + (j - i); }  // upper-tri index of the 7x7, i <= j
+constexpr int kTdSums = kLmSums<7>;  // 28 upper-tri of the 7x7 H (tx ty tz rx ry rz td, row-major, i <= j) + 7 g + 1 cost
+constexpr int kTdFrameDoubles = 8;         // per frame: n[3], mdot[3], cdot, unused
+constexpr int kKnotDoubles = 7;            // per knot: q_ac (x, y, z, w), t_ac
 
 // ---- the trajectory ----------------------------------------------------------------------------------------------------------
 
@@ -156,7 +154,7 @@ CLC_HD void expand_lm_td(const double* n, const double* m, double c, const doubl
   for (int k = 0; k < kNumSums; ++k) o[k] = 0.0;
   expand_lm(plane, m, c, s2, S, loss, cost_term, a2, o);
   for (int i = 0; i < 6; ++i)
-    for (int j = i; j < 6; ++j) out[tri7(i, j)] += o[tri(i, j)];
+    for (int j = i; j < 6; ++j) out[tri<7>(i, j)] += o[tri(i, j)];
   for (int i = 0; i < 6; ++i) out[28 + i] += o[21 + i];
   out[35] += o[27];
   const double S0 = S[0];
@@ -172,271 +170,22 @@ CLC_HD void expand_lm_td(const double* n, const double* m, double c, const doubl
   const double E0 = m[0] * S1[0] + m[1] * S1[1] + m[2] * S1[2] + c * S0;
   double smx[3];
   cross3(Sm, m, smx);
-  for (int i = 0; i < 3; ++i) out[tri7(i, 6)] += s2 * n[i] * Ew;
-  for (int i = 0; i < 3; ++i) out[tri7(3 + i, 6)] += s2 * smx[i];
-  out[tri7(6, 6)] += s2 * (md[0] * Sm[0] + md[1] * Sm[1] + md[2] * Sm[2] + cd * Ew);
+  for (int i = 0; i < 3; ++i) out[tri<7>(i, 6)] += s2 * n[i] * Ew;
+  for (int i = 0; i < 3; ++i) out[tri<7>(3 + i, 6)] += s2 * smx[i];
+  out[tri<7>(6, 6)] += s2 * (md[0] * Sm[0] + md[1] * Sm[1] + md[2] * Sm[2] + cd * Ew);
   out[34] += s2 * (md[0] * v[0] + md[1] * v[1] + md[2] * v[2] + cd * E0);
 }
 
-// ---- Ceres' LM on two parameter blocks: the pose (local size 6) and td (a 1-vector) --------------------------------------------
-// lm_update's state machine over 7 columns: x = (pose7, td), the parameter tolerance on the 8-vector, gradient_max_norm =
-// max(|x - Plus(x, -g)|_inf over the pose, |g_td|).  fixed_mask bit 6 holds td (its start bits kept), bits 0-5 as in lm_hold.
+// ---- Ceres' LM on two parameter blocks, the pose (local size 6) and td (a 1-vector): clc_lm.cuh's state machine at D = 7 -------
 
-struct LmCoreTd {
-  int done;  // as LmCore
-  int phase;
-  int iteration;
-  int num_invalid;
-  int reuse_diagonal;
-  int n_trace;
-  int num_successful;
-  int num_unsuccessful;
-  int sweeps;
-  int pad0;
-  double x[8];     // pose7, td
-  double cand[8];  // the point the next sweep evaluates
-  double x_cost, x_norm;
-  double H[28], g[7];
-  double scale[7], diag[7];
-  double radius, decrease_factor, model_cost_change;
-  double initial_cost;
-  clc_lm_options opt;
-};
-static_assert(sizeof(LmCoreTd) % 8 == 0, "LmCoreTd is copied as 8-byte words");
-constexpr int kLmCoreTdWords = (int)(sizeof(LmCoreTd) / 8);
-
-CLC_HD double norm8(const double* a) {
-  double s = 0.0;
-  for (int i = 0; i < 8; ++i) s += a[i] * a[i];
-  return sqrt(s);
-}
-
-CLC_HD double gradient_max_norm_td(const double* x, const double* g) {
-  const double m = gradient_max_norm(x, g), a = fabs(g[6]);
-  return a > m ? a : m;
-}
-
-// Cholesky solve of the SPD 7x7 system A y = b (chol6_solve's arithmetic).  false if not positive definite.
-CLC_HD bool chol7_solve(const double* A, const double* b, double* y) {
-  constexpr int N = 7;
-  double L[N * N], inv[N];
-  bool ok = true;
-#pragma unroll
-  for (int j = 0; j < N; ++j) {
-    double s = A[j * N + j];
-#pragma unroll
-    for (int k = 0; k < j; ++k) s -= L[j * N + k] * L[j * N + k];
-    ok = ok && (s > 0.0);
-    const double d = sqrt(s);
-    L[j * N + j] = d;
-    inv[j] = 1.0 / d;
-#pragma unroll
-    for (int i = j + 1; i < N; ++i) {
-      double t = A[i * N + j];
-#pragma unroll
-      for (int k = 0; k < j; ++k) t -= L[i * N + k] * L[j * N + k];
-      L[i * N + j] = t * inv[j];
-    }
-  }
-  if (!ok) return false;
-  double z[N];
-#pragma unroll
-  for (int i = 0; i < N; ++i) {
-    double s = b[i];
-#pragma unroll
-    for (int k = 0; k < i; ++k) s -= L[i * N + k] * z[k];
-    z[i] = s * inv[i];
-  }
-#pragma unroll
-  for (int i = N - 1; i >= 0; --i) {
-    double s = z[i];
-#pragma unroll
-    for (int k = i + 1; k < N; ++k) s -= L[k * N + i] * y[k];
-    y[i] = s * inv[i];
-  }
-  return true;
-}
-
-// lm_hold over 7 columns
-CLC_HD void lm_hold_td(LmCoreTd* s, int fixed) {
-#pragma unroll 1
-  for (int k = 0; k < 7; ++k) {
-    if (!(fixed >> k & 1)) continue;
-#pragma unroll 1
-    for (int j = 0; j < 7; ++j) s->H[j < k ? tri7(j, k) : tri7(k, j)] = 0.0;
-    s->H[tri7(k, k)] = 1.0;
-    s->g[k] = 0.0;
-  }
-}
-
-// a held translation coordinate or td keeps the bits of x
-CLC_HD void lm_hold_cand_td(LmCoreTd* s, int fixed) {
-#pragma unroll 1
-  for (int k = 0; k < 3; ++k)
-    if (fixed >> k & 1) s->cand[k] = s->x[k];
-  if (fixed >> 6 & 1) s->cand[7] = s->x[7];
-}
-
-CLC_HD void lm_record(LmCoreTd* s, TraceRows trace, const clc_lm_iteration& it) {
-  if (s->n_trace < trace.cap) trace.rows[s->n_trace] = it;
-  s->n_trace++;
-}
+using LmCoreTd = LmCoreN<7>;
 
 CLC_HD void lm_init_td(LmCoreTd* s, const double* pose7, double td, const clc_lm_options& opt) {
-  s->done = 0; s->phase = 0; s->iteration = 0; s->num_invalid = 0; s->reuse_diagonal = 0; s->n_trace = 0;
-  s->num_successful = 0; s->num_unsuccessful = 0; s->sweeps = 0; s->pad0 = 0;
-  for (int i = 0; i < 7; ++i) { s->x[i] = pose7[i]; s->cand[i] = pose7[i]; }
-  s->x[7] = td; s->cand[7] = td;
-  s->x_cost = 0.0;
-  s->x_norm = norm8(s->x);
-  s->radius = opt.initial_trust_region_radius;
-  s->decrease_factor = 2.0;
-  s->model_cost_change = 0.0;
-  s->initial_cost = 0.0;
-  s->opt = opt;
+  const double x8[8] = {pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6], td};
+  lm_init(s, x8, opt);
 }
 
-// lm_update on the kTdSums sums of the sweep that has just evaluated s->cand.
-CLC_HD void lm_update_td(LmCoreTd* s, TraceRows trace, const double* sums) {
-  if (s->done) return;
-  s->sweeps++;
-  const clc_lm_options& o = s->opt;
-  clc_lm_iteration last;
-  last.reserved = 0;
-  bool sums_ok = true;
-  for (int i = 0; i < kTdSums; ++i) sums_ok = sums_ok && is_finite(sums[i]);
-  if (s->phase == 0) {
-    if (!sums_ok) { s->done = CLC_TERM_FAILURE; return; }
-    s->x_cost = sums[35];
-    for (int i = 0; i < 28; ++i) s->H[i] = sums[i];
-    for (int i = 0; i < 7; ++i) s->g[i] = sums[28 + i];
-    if (o.fixed_mask) lm_hold_td(s, o.fixed_mask);
-    for (int k = 0; k < 7; ++k) s->scale[k] = o.jacobi_scaling ? 1.0 / (1.0 + sqrt(s->H[tri7(k, k)])) : 1.0;
-    s->initial_cost = s->x_cost;
-    last.iteration = 0; last.step_is_valid = 1; last.step_is_successful = 1;
-    last.cost = s->x_cost; last.cost_change = 0.0; last.gradient_max_norm = gradient_max_norm_td(s->x, s->g);
-    last.step_norm = 0.0; last.relative_decrease = 0.0; last.trust_region_radius = s->radius;
-  } else {
-    const double cand_cost = sums_ok ? sums[35] : DBL_MAX;
-    last.iteration = s->iteration + 1; last.step_is_valid = 1; last.step_is_successful = 0;
-    double d[8];
-    for (int i = 0; i < 8; ++i) d[i] = s->x[i] - s->cand[i];
-    last.step_norm = norm8(d);
-    last.cost_change = s->x_cost - cand_cost;
-    last.cost = cand_cost;
-    last.gradient_max_norm = 0.0; last.relative_decrease = 0.0; last.trust_region_radius = s->radius;
-    if (last.step_norm <= o.parameter_tolerance * (s->x_norm + o.parameter_tolerance)) {
-      s->done = CLC_TERM_CONVERGENCE_PARAMETER;
-      lm_record(s, trace, last);
-      return;
-    }
-    if (fabs(last.cost_change) <= o.function_tolerance * s->x_cost) {
-      s->done = CLC_TERM_CONVERGENCE_FUNCTION;
-      lm_record(s, trace, last);
-      return;
-    }
-    last.relative_decrease = last.cost_change / s->model_cost_change;
-    if (last.relative_decrease > o.min_relative_decrease) {
-      for (int i = 0; i < 8; ++i) s->x[i] = s->cand[i];
-      s->x_norm = norm8(s->x);
-      s->x_cost = cand_cost;
-      for (int i = 0; i < 28; ++i) s->H[i] = sums[i];
-      for (int i = 0; i < 7; ++i) s->g[i] = sums[28 + i];
-      if (o.fixed_mask) lm_hold_td(s, o.fixed_mask);
-      last.step_is_successful = 1;
-      last.gradient_max_norm = gradient_max_norm_td(s->x, s->g);
-      const double q = 2.0 * last.relative_decrease - 1.0;
-      double den = 1.0 - q * q * q;
-      if (den < 1.0 / 3.0) den = 1.0 / 3.0;
-      s->radius = s->radius / den;
-      if (s->radius > o.max_trust_region_radius) s->radius = o.max_trust_region_radius;
-      s->decrease_factor = 2.0;
-      s->reuse_diagonal = 0;
-    } else {
-      s->radius = s->radius / s->decrease_factor;
-      s->decrease_factor *= 2.0;
-      s->reuse_diagonal = 1;
-    }
-  }
-
-  for (;;) {
-    if (last.step_is_successful) s->num_successful++; else s->num_unsuccessful++;
-    last.trust_region_radius = s->radius;
-    lm_record(s, trace, last);
-    s->iteration = last.iteration;
-    if (last.iteration >= o.max_num_iterations) { s->done = CLC_TERM_NO_CONVERGENCE; return; }
-    if (last.step_is_successful && last.gradient_max_norm <= o.gradient_tolerance) {
-      s->done = CLC_TERM_CONVERGENCE_GRADIENT;
-      return;
-    }
-    if (!(s->radius > o.min_trust_region_radius)) { s->done = CLC_TERM_CONVERGENCE_MIN_RADIUS; return; }
-
-    double Hs[49], gs[7], A[49], step[7];
-#pragma unroll
-    for (int i = 0; i < 7; ++i) {
-      gs[i] = s->scale[i] * s->g[i];
-#pragma unroll
-      for (int j = i; j < 7; ++j) {
-        const double v = s->scale[i] * s->scale[j] * s->H[tri7(i, j)];
-        Hs[i * 7 + j] = v;
-        Hs[j * 7 + i] = v;
-      }
-    }
-    if (!s->reuse_diagonal)
-#pragma unroll
-      for (int k = 0; k < 7; ++k) {
-        double dd = Hs[k * 7 + k];
-        dd = dd > o.min_lm_diagonal ? dd : o.min_lm_diagonal;
-        dd = dd < o.max_lm_diagonal ? dd : o.max_lm_diagonal;
-        s->diag[k] = dd;
-      }
-#pragma unroll
-    for (int i = 0; i < 49; ++i) A[i] = Hs[i];
-    const double inv_radius = 1.0 / s->radius;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) A[k * 7 + k] += s->diag[k] * inv_radius;
-    bool ok = chol7_solve(A, gs, step);
-    s->reuse_diagonal = 1;
-#pragma unroll
-    for (int k = 0; k < 7; ++k) {
-      if (!is_finite(step[k])) ok = false;
-      step[k] = -step[k];
-    }
-    double mcc = 0.0;
-    if (ok) {
-      double gs_s = 0.0, sHs = 0.0;
-#pragma unroll
-      for (int i = 0; i < 7; ++i) {
-        gs_s += gs[i] * step[i];
-        double r = 0.0;
-#pragma unroll
-        for (int j = 0; j < 7; ++j) r += Hs[i * 7 + j] * step[j];
-        sHs += step[i] * r;
-      }
-      mcc = -gs_s - 0.5 * sHs;
-    }
-    if (!(ok && mcc > 0.0)) {
-      if (++s->num_invalid >= o.max_num_consecutive_invalid_steps) { s->done = CLC_TERM_FAILURE; return; }
-      s->radius = s->radius / s->decrease_factor;
-      s->decrease_factor *= 2.0;
-      s->reuse_diagonal = 1;
-      const double prev_gmax = last.gradient_max_norm;
-      last.iteration = s->iteration + 1; last.step_is_valid = 0; last.step_is_successful = 0;
-      last.cost = s->x_cost; last.cost_change = 0.0; last.gradient_max_norm = prev_gmax;
-      last.step_norm = 0.0; last.relative_decrease = 0.0;
-      continue;
-    }
-    s->num_invalid = 0;
-    double delta[7];
-    for (int k = 0; k < 7; ++k) delta[k] = step[k] * s->scale[k];
-    pose_plus(s->x, delta, s->cand);
-    s->cand[7] = s->x[7] + delta[6];
-    if (o.fixed_mask) lm_hold_cand_td(s, o.fixed_mask);
-    s->model_cost_change = mcc;
-    s->phase = 1;
-    return;
-  }
-}
+CLC_HD void lm_update_td(LmCoreTd* s, TraceRows trace, const double* sums) { lm_update(s, trace, sums); }
 
 }  // namespace clc
 
@@ -489,49 +238,6 @@ __global__ void clc_time_fixup_kernel(ProblemView pv, const double* __restrict__
   expand_lm_td(n, m, consts[f * 4 + 3], md, tf[6], s2, S, LOSS, cost_term, pv.a2, out);
 #pragma unroll
   for (int k = 0; k < kTdSums; ++k) row[k] = out[k];
-}
-
-// Level 1 at width kTdSums: one warp per chunk, lane k adds outputs k and k + 32 of the chunk's rows in frame order.
-__global__ void __launch_bounds__(32 * kSegWarpsPerBlock)
-clc_time_chunk_kernel(const double* __restrict__ rows, const int64_t* __restrict__ chunk_offsets, int64_t n_chunks, const int* done,
-                      double* __restrict__ partials) {
-  const int64_t ch = (int64_t)blockIdx.x * kSegWarpsPerBlock + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (ch >= n_chunks || (done != nullptr && *done != 0)) return;
-  const int64_t a = chunk_offsets[ch], b = chunk_offsets[ch + 1];
-  for (int k = lane; k < kTdSums; k += 32) {
-    double acc = 0.0;
-    for (int64_t r = a; r < b; ++r) acc += rows[r * kTdSums + k];
-    partials[ch * kTdSums + k] = acc;
-  }
-}
-
-// Level 2 + LM, one warp: the chunk partials in chunk order into sums (may be nullptr); with a core, lane 0 then runs lm_update_td
-// on it, staged in shared memory, and raises `done` when it terminates.
-__global__ void __launch_bounds__(32)
-clc_time_lm_kernel(const double* __restrict__ partials, int64_t n_chunks, double* sums, LmCoreTd* core, clc_lm_iteration* trace,
-                   int trace_cap, int* done) {
-  __shared__ unsigned long long s_core[kLmCoreTdWords];
-  __shared__ double s_sums[kTdSums];
-  const int lane = threadIdx.x & 31;
-  if (done != nullptr && *done != 0) return;
-  for (int k = lane; k < kTdSums; k += 32) {
-    double acc = 0.0;
-    for (int64_t c = 0; c < n_chunks; ++c) acc += partials[c * kTdSums + k];
-    s_sums[k] = acc;
-    if (sums != nullptr) sums[k] = acc;
-  }
-  if (core == nullptr) return;
-  unsigned long long* g_core = reinterpret_cast<unsigned long long*>(core);
-  for (int k = lane; k < kLmCoreTdWords; k += 32) s_core[k] = g_core[k];
-  __syncwarp();
-  if (lane == 0) {
-    LmCoreTd* s = reinterpret_cast<LmCoreTd*>(s_core);
-    lm_update_td(s, TraceRows{trace, trace_cap}, s_sums);
-    if (s->done != 0) *done = 1;
-  }
-  __syncwarp();
-  for (int k = lane; k < kLmCoreTdWords; k += 32) g_core[k] = s_core[k];
 }
 
 }  // namespace clc
