@@ -15,6 +15,7 @@ from .api import (  # noqa: F401
     Group,
     Oberserve,
     Problem,
+    Selection,
     T_to_pose7,
     comm_unique_id,
     debug_pack,
@@ -23,6 +24,7 @@ from .api import (  # noqa: F401
     launch_count,
     marshal,
     pose7_to_T,
+    select_frames_from_report,
     shard_range,
     upload_stats,
 )
@@ -30,5 +32,5 @@ from .api import (  # noqa: F401
 __all__ = [
     "CamLaserCalClosedSolution", "CamLaserCalibration", "LineFittingCeres", "ClcError", "Comm", "Group", "Oberserve", "Problem", "T_to_pose7",
     "comm_unique_id", "default_options", "launch_count", "marshal", "pose7_to_T", "shard_range", "debug_pack", "upload_stats",
-    "FRAME_ROW_DTYPE", "frame_influence",
+    "FRAME_ROW_DTYPE", "frame_influence", "Selection", "select_frames_from_report",
 ]

@@ -142,6 +142,16 @@ class FrameRow(C.Structure):
     ]
 
 
+class SelectDesc(C.Structure):
+    """clc_select_desc."""
+    _fields_ = [
+        ("budget", C.c_int64),
+        ("min_gain", C.c_double),
+        ("fixed_mask", C.c_int),
+        ("state", C.POINTER(C.c_uint8)),
+    ]
+
+
 TERMINATION = {
     0: "RUNNING",
     1: "CONVERGENCE_FUNCTION",
@@ -174,6 +184,12 @@ SIGNATURES = {
     "clc_group_information": (C.c_int, [_P, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     "clc_group_closed_form": (C.c_int, [_P, c_double_p, C.POINTER(C.c_int), c_double_p, c_double_p]),
     "clc_group_frame_report": (C.c_int, [_P, c_double_p, _P]),
+    "clc_select_frames": (C.c_int, [_P, c_double_p, C.POINTER(SelectDesc), c_int64_p, c_int64_p, c_double_p, C.POINTER(C.c_uint8)]),
+    "clc_select_frames_rows": (C.c_int, [C.c_int, C.c_int64, _P, C.POINTER(SelectDesc), c_int64_p, c_int64_p, c_double_p,
+                                         C.POINTER(C.c_uint8)]),
+    "clc_group_select_frames": (C.c_int, [_P, c_double_p, C.POINTER(SelectDesc), c_int64_p, c_int64_p, c_double_p,
+                                          C.POINTER(C.c_uint8)]),
+    "clc_bench_select": (C.c_int, [_P, c_double_p, C.POINTER(SelectDesc), C.c_int, C.POINTER(C.c_float), c_int64_p]),
     "clc_problem_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.POINTER(_P)]),
     "clc_group_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.POINTER(_P)]),
     "clc_problem_trim": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(_P)]),

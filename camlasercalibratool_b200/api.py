@@ -10,11 +10,12 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass, field
+from typing import NamedTuple
 
 import numpy as np
 
 from . import _lib
-from ._lib import ClcError, GatherDesc, LmIteration, LmOptions, LmSummary, ProblemDesc, SyntheticDesc, TERMINATION
+from ._lib import ClcError, GatherDesc, LmIteration, LmOptions, LmSummary, ProblemDesc, SelectDesc, SyntheticDesc, TERMINATION
 
 
 def _dp(a):
@@ -168,6 +169,60 @@ def _keep_mask(keep, n_frames):
     if keep.shape != (n_frames,):
         raise ValueError(f"keep must have shape ({n_frames},), not {keep.shape}")
     return np.ascontiguousarray(keep, dtype=np.uint8)
+
+
+class Selection(NamedTuple):
+    """A frame selection (clc_select_frames): order [n_selected] the picked frames in pick order, gain [n_selected] the
+    information each added (nats), keep [n_frames] the forced and the picked frames -- the mask subset() takes."""
+    order: np.ndarray
+    gain: np.ndarray
+    keep: np.ndarray
+
+
+def _select_args(n_frames, budget, min_gain, candidates, forced, fixed):
+    """The checked arguments of a selection -> (clc_select_desc, the uint8 states it points to or None), before any device work:
+    budget an integer >= 0, min_gain finite and >= 0, candidates / forced boolean masks of shape (n_frames,) (a frame in both is
+    forced), fixed names of FIXED_NAMES."""
+    if isinstance(budget, (bool, np.bool_)) or not isinstance(budget, (int, np.integer)):
+        raise TypeError(f"budget must be an integer, not {type(budget).__name__}")
+    if budget < 0:
+        raise ValueError(f"budget must be >= 0, not {budget}")
+    min_gain = float(min_gain)
+    if not (np.isfinite(min_gain) and min_gain >= 0.0):
+        raise ValueError(f"min_gain must be finite and >= 0, not {min_gain!r}")
+    mask = fixed_mask(fixed)
+    state = None
+    if candidates is not None or forced is not None:
+        state = np.ones(n_frames, dtype=np.uint8)
+        if candidates is not None:
+            state[_keep_mask(candidates, n_frames) == 0] = 0
+        if forced is not None:
+            state[_keep_mask(forced, n_frames) != 0] = 2
+    d = SelectDesc()
+    d.budget, d.min_gain, d.fixed_mask = int(budget), min_gain, mask
+    d.state = state.ctypes.data_as(C.POINTER(C.c_uint8)) if state is not None else None
+    return d, state
+
+
+def _select(fn, args, n_frames, desc, what):
+    cap = max(min(int(desc.budget), n_frames), 1)
+    order, gain, keep = np.zeros(cap, dtype=np.int64), np.zeros(cap), np.zeros(max(n_frames, 1), dtype=np.uint8)
+    n = C.c_int64()
+    _lib.check(fn(*args, C.byref(desc), C.byref(n), _ip(order), _dp(gain), keep.ctypes.data_as(C.POINTER(C.c_uint8))), what)
+    return Selection(order[:n.value].copy(), gain[:n.value].copy(), keep[:n_frames].astype(bool))
+
+
+def select_frames_from_report(rows, budget, min_gain=0.0, candidates=None, forced=None, fixed=(), device=-1):
+    """Problem.select_frames on report rows the caller holds (clc_select_frames_rows): rows is a FRAME_ROW_DTYPE array (a
+    frame_report, or constructed rows; only H21 is read), uploaded once to `device` (-1: the current one)."""
+    rows = np.asarray(rows)
+    if rows.dtype != FRAME_ROW_DTYPE or rows.ndim != 1:
+        raise TypeError(f"rows must be a 1-D array of FRAME_ROW_DTYPE, not {rows.dtype} of shape {rows.shape}")
+    rows = np.ascontiguousarray(rows)
+    n = rows.shape[0]
+    desc, _state = _select_args(n, budget, min_gain, candidates, forced, fixed)
+    return _select(_lib.load().clc_select_frames_rows, (int(device), n, rows.ctypes.data_as(C.c_void_p)), n, desc,
+                   "clc_select_frames_rows")
 
 
 # the loss kinds of set_loss (include/clc_b200.h CLC_LOSS_*)
@@ -506,6 +561,18 @@ class Problem:
         information()'s chi."""
         return _frame_report(self._L.clc_frame_report, self._h, self.sizes()[0], pose7, "clc_frame_report")
 
+    def select_frames(self, pose7, budget, min_gain=0.0, candidates=None, forced=None, fixed=()):
+        """Greedy D-optimal selection of at most `budget` frames by the information they add about the extrinsic at pose7
+        (clc_select_frames; the rule is in include/clc_b200.h).  candidates: boolean mask of the frames that may be picked (None:
+        all); forced: boolean mask of frames kept from the start and never picked (they count as already selected); fixed: names
+        of coordinates left out of the information, as default_options takes them.  Stops early once the best gain is <= min_gain
+        nats or no candidate is left.  Returns a Selection (order, gain, keep); keep is the mask subset() takes:
+        ``with p.subset(p.select_frames(x, 200).keep) as q: q.solve(x)``."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        n = self.sizes()[0]
+        desc, _state = _select_args(n, budget, min_gain, candidates, forced, fixed)
+        return _select(self._L.clc_select_frames, (self._h, _dp(pose7)), n, desc, "clc_select_frames")
+
     # ---- independent solves over runs of frames (segments) ----
     def eval_segments(self, seg_offsets, poses):
         """eval() of every segment [seg_offsets[s], seg_offsets[s + 1]) of the frames at its own pose poses[s], from ONE shared
@@ -649,6 +716,14 @@ class Problem:
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_frame_report(self._h, _dp(pose7), int(n), int(bool(flush_l2)), ms), "clc_bench_frame_report")
         return np.array(ms[:], dtype=np.float64)
+
+    def bench_select(self, pose7, budget, n, min_gain=0.0, fixed=()):
+        """Device time of n selections on one report's device rows (clc_bench_select), ms each, and the picks of the last run."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        desc, _state = _select_args(self.sizes()[0], budget, min_gain, None, None, fixed)
+        ms, k = (C.c_float * n)(), C.c_int64()
+        _lib.check(self._L.clc_bench_select(self._h, _dp(pose7), C.byref(desc), int(n), ms, C.byref(k)), "clc_bench_select")
+        return np.array(ms[:], dtype=np.float64), k.value
 
     def bench_segments(self, seg_offsets, poses, n, flush_l2=True):
         """Device time of n iterations of the segmented calls (frame constants, segment sweep, fix-up, two-level reduction;
@@ -811,6 +886,14 @@ class Group:
     def frame_report(self, pose7):
         """Problem.frame_report over every shard, rows in the global frame order (clc_group_frame_report)."""
         return _frame_report(self._L.clc_group_frame_report, self._h, self.sizes()[1], pose7, "clc_group_frame_report")
+
+    def select_frames(self, pose7, budget, min_gain=0.0, candidates=None, forced=None, fixed=()):
+        """Problem.select_frames over every shard (clc_group_select_frames): the frame_report rows in the global frame order,
+        selected on the group's first device; order and keep are in the global frame order."""
+        pose7 = np.ascontiguousarray(pose7, dtype=np.float64)
+        n = self.sizes()[1]
+        desc, _state = _select_args(n, budget, min_gain, candidates, forced, fixed)
+        return _select(self._L.clc_group_select_frames, (self._h, _dp(pose7)), n, desc, "clc_group_select_frames")
 
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()

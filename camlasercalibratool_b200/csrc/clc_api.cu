@@ -25,6 +25,7 @@
 #include "clc_l2_plan.h"
 #include "clc_linefit.cuh"
 #include "clc_segments.cuh"
+#include "clc_select.cuh"
 #include "clc_small.cuh"
 #include "clc_subset.cuh"
 #include "clc_subset_plan.h"
@@ -1448,29 +1449,37 @@ int lm_batch(const clc_lm_options& opt, int launched, int max_sweeps) {
   return std::min(launched == 0 ? 2 * opt.iterations_per_sync : opt.iterations_per_sync, max_sweeps - launched);
 }
 
-// The host loop of a batched on-device solve (segments, starts, time offset): enqueue() queues one LM iteration, in batches of
-// lm_batch, until lm_max_sweeps are queued or the device counter *d_running of solves still running reads 0 after a batch.  The
-// device time from the first iteration to the end of the last into *ms.
-int lm_batches(clc_problem* p, const clc_lm_options& opt, const int* d_running, const std::function<int()>& enqueue, float* ms) {
-  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
-  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
-  CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
-  const int max_sweeps = lm_max_sweeps(opt);
-  for (int launched = 0; launched < max_sweeps;) {
-    const int batch = lm_batch(opt, launched, max_sweeps);
-    for (int i = 0; i < batch; ++i) {
+// The host loop of every batched on-device iteration: enqueue() queues one launch, in batches of batch(launched), until
+// max_launches are queued or the device counter *d_running reads 0 after a batch (h_flag: pinned host memory for it).  The device
+// time from the first launch to the end of the last into *ms.
+int poll_batches(cudaStream_t stream, cudaEvent_t ev0, cudaEvent_t ev1, int* h_flag, int64_t max_launches,
+                 const std::function<int(int64_t)>& batch_of, const int* d_running, const std::function<int()>& enqueue, float* ms) {
+  CLC_CUDA(cudaEventRecord(ev0, stream));
+  for (int64_t launched = 0; launched < max_launches;) {
+    const int64_t batch = batch_of(launched);
+    for (int64_t i = 0; i < batch; ++i) {
       const int rc = enqueue();
       if (rc != CLC_OK) return rc;
     }
     launched += batch;
-    CLC_CUDA(cudaMemcpyAsync(p->h_done, d_running, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-    CLC_CUDA(sync_stream_low_latency(p->stream));
-    if (*p->h_done == 0) break;  // no solve is running
+    CLC_CUDA(cudaMemcpyAsync(h_flag, d_running, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CLC_CUDA(sync_stream_low_latency(stream));
+    if (*h_flag == 0) break;  // nothing is running
   }
-  CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
-  CLC_CUDA(cudaEventSynchronize(p->ev1));
-  CLC_CUDA(cudaEventElapsedTime(ms, p->ev0, p->ev1));
+  CLC_CUDA(cudaEventRecord(ev1, stream));
+  CLC_CUDA(cudaEventSynchronize(ev1));
+  CLC_CUDA(cudaEventElapsedTime(ms, ev0, ev1));
   return CLC_OK;
+}
+
+// The host loop of a batched on-device solve (segments, starts, time offset): poll_batches with one LM iteration per launch, in
+// batches of lm_batch, up to lm_max_sweeps.
+int lm_batches(clc_problem* p, const clc_lm_options& opt, const int* d_running, const std::function<int()>& enqueue, float* ms) {
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  const int max_sweeps = lm_max_sweeps(opt);
+  return poll_batches(p->stream, p->ev0, p->ev1, p->h_done, max_sweeps,
+                      [&](int launched) { return lm_batch(opt, launched, max_sweeps); }, d_running, enqueue, ms);
 }
 
 extern "C++" {
@@ -2946,6 +2955,226 @@ int clc_group_closed_form(clc_group* g, double Tlc16[16], int* unobservable, dou
 int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* rows) {
   if (!g || g->problems.empty() || !pose7 || (!rows && g->n_frames > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
   return frame_report_all(g->problems.data(), (int)g->problems.size(), pose7, rows);
+}
+
+// ---- greedy D-optimal frame selection (clc_select.cuh) --------------------------------------------------------------------
+// One selection on a stream: the rows (report rows on the device, kRowDoubles apart) through the sum, init and scale kernels, then
+// one step launch per pick, in batches of kSelectBatch between host polls of SelState::running.  The outputs come back in one
+// copy at the end.
+
+namespace {
+
+// Step launches between two host polls.  A selection that runs to its budget (the usual case) costs one poll per batch; one that
+// stops early queues at most kSelectBatch - 1 launches that return at once.
+constexpr int64_t kSelectBatch = 64;
+
+static_assert(clc::kSelectRidge == CLC_SELECT_RIDGE, "the ridge of the header");
+const char* const kCoordNames[6] = {"tx", "ty", "tz", "rx", "ry", "rz"};
+
+// the checks of every selection entry point, before any device work
+int select_check(const clc_select_desc* desc, int64_t n_frames, int64_t* n_selected, int64_t* order, double* gain, uint8_t* keep) {
+  if (!desc) return fail(CLC_ERR_INVALID, "NULL select descriptor");
+  if (desc->budget < 0) return fail(CLC_ERR_INVALID, "budget must be >= 0");
+  if (!(desc->min_gain >= 0.0) || !clc::is_finite(desc->min_gain)) return fail(CLC_ERR_INVALID, "min_gain must be finite and >= 0");
+  if (desc->fixed_mask < 0 || desc->fixed_mask >= 63)
+    return fail(CLC_ERR_INVALID, "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)");
+  if (desc->state && n_frames > 0)
+    for (int64_t f = 0; f < n_frames; ++f)
+      if (desc->state[f] > 2) return fail(CLC_ERR_INVALID, "a frame state must be 0 (excluded), 1 (candidate) or 2 (forced)");
+  const int64_t cap = std::min(desc->budget, n_frames);
+  if (!n_selected || (cap > 0 && (!order || !gain)) || (n_frames > 0 && !keep)) return fail(CLC_ERR_INVALID, "NULL output");
+  return CLC_OK;
+}
+
+// where a selection runs: a stream on a device, two events and pinned host memory for the poll
+struct SelectStream {
+  cudaStream_t stream;
+  cudaEvent_t ev0, ev1;
+  int* h_flag;
+  int num_sms;
+};
+
+// The selection on n_frames rows at d_rows (device memory on the current device), desc already checked.  *ms (may be NULL): device
+// time from the sum kernel to the end of the last step, the host polls included.
+int select_run(const SelectStream& ss, const double* d_rows, int64_t n, const clc_select_desc* desc, int64_t* n_selected,
+               int64_t* order, double* gain, uint8_t* keep, float* ms) {
+  *n_selected = 0;
+  if (n == 0) {
+    if (ms) *ms = 0.f;
+    return CLC_OK;
+  }
+  clc::SelFree fr{};
+  fr.d = 0;
+  for (int k = 0; k < 6; ++k)
+    if (!((desc->fixed_mask >> k) & 1)) fr.idx[fr.d++] = k;
+  const int np = fr.d * (fr.d + 1) / 2;
+  const int64_t cap = std::min(desc->budget, n);
+  const int64_t blocks = (n + clc::kSelThreads - 1) / clc::kSelThreads;
+  int occ = 0;
+  CLC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, clc::clc_select_step_kernel, clc::kSelThreads, 0));
+  const int64_t step_grid = std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)ss.num_sms * std::max(occ, 1)));
+  // one allocation: packed blocks, partials, state, bests, order, gain, caller states, status, keep
+  auto up8 = [](size_t b) { return (b + 7) & ~(size_t)7; };
+  size_t off = 0;
+  const size_t o_packed = off; off += up8(sizeof(double) * (size_t)np * n);
+  const size_t o_part = off;   off += up8(sizeof(double) * (size_t)clc::kSelSums * blocks);
+  const size_t o_state = off;  off += up8(sizeof(clc::SelState));
+  const size_t o_best = off;   off += up8(sizeof(clc::SelBest) * (size_t)step_grid);
+  const size_t o_order = off;  off += up8(sizeof(int64_t) * (size_t)std::max<int64_t>(cap, 1));
+  const size_t o_gain = off;   off += up8(sizeof(double) * (size_t)std::max<int64_t>(cap, 1));
+  const size_t o_in = off;     off += up8(desc->state ? (size_t)n : 0);
+  const size_t o_status = off; off += up8((size_t)n);
+  const size_t o_keep = off;   off += up8((size_t)n);
+  char* buf = nullptr;
+  CLC_CUDA(cudaMallocAsync(&buf, off, ss.stream));
+  double* packed = reinterpret_cast<double*>(buf + o_packed);
+  double* partials = reinterpret_cast<double*>(buf + o_part);
+  clc::SelState* st = reinterpret_cast<clc::SelState*>(buf + o_state);
+  clc::SelBest* bests = reinterpret_cast<clc::SelBest*>(buf + o_best);
+  int64_t* d_order = reinterpret_cast<int64_t*>(buf + o_order);
+  double* d_gain = reinterpret_cast<double*>(buf + o_gain);
+  uint8_t* d_in = desc->state ? reinterpret_cast<uint8_t*>(buf + o_in) : nullptr;
+  uint8_t* status = reinterpret_cast<uint8_t*>(buf + o_status);
+  uint8_t* d_keep = reinterpret_cast<uint8_t*>(buf + o_keep);
+  struct FreeOnExit {
+    char* b;
+    cudaStream_t s;
+    ~FreeOnExit() { cudaFreeAsync(b, s); }
+  } free_on_exit{buf, ss.stream};
+  if (d_in) CLC_CUDA(cudaMemcpyAsync(d_in, desc->state, (size_t)n, cudaMemcpyHostToDevice, ss.stream));
+  CLC_CUDA(cudaEventRecord(ss.ev0, ss.stream));
+  clc::clc_select_sum_kernel<<<(unsigned)blocks, clc::kSelThreads, 0, ss.stream>>>(d_rows, clc::kRowDoubles, clc::kRowH, n, d_in, fr,
+                                                                                   packed, status, d_keep, partials);
+  CLC_LAUNCH_CHECK();
+  clc::clc_select_init_kernel<<<1, 64, 0, ss.stream>>>(partials, blocks, fr, desc->min_gain, desc->budget, st);
+  CLC_LAUNCH_CHECK();
+  clc::clc_select_scale_kernel<<<(unsigned)blocks, clc::kSelThreads, 0, ss.stream>>>(packed, n, fr.d, st);
+  CLC_LAUNCH_CHECK();
+  float steps_ms = 0.f;
+  int rc = poll_batches(ss.stream, ss.ev0, ss.ev1, ss.h_flag, cap + 1,
+                        [&](int64_t launched) { return std::min(kSelectBatch, cap + 1 - launched); }, &st->running,
+                        [&]() {
+                          clc::clc_select_step_kernel<<<(unsigned)step_grid, clc::kSelThreads, 0, ss.stream>>>(
+                              packed, n, fr.d, status, st, bests, d_order, d_gain, d_keep);
+                          CLC_LAUNCH_CHECK();
+                          return CLC_OK;
+                        },
+                        &steps_ms);
+  if (rc != CLC_OK) return rc;
+  if (ms) *ms = steps_ms;
+  clc::SelState h;
+  CLC_CUDA(cudaMemcpyAsync(&h, st, sizeof(h), cudaMemcpyDeviceToHost, ss.stream));
+  CLC_CUDA(cudaStreamSynchronize(ss.stream));
+  if (h.status != 0)
+    return fail(CLC_ERR_STATE, std::string("select: no usable frame observes coordinate ") + kCoordNames[h.status - 1] +
+                                   " (its total information is not positive and finite); hold it in fixed_mask");
+  if (h.n_sel > 0) {
+    CLC_CUDA(cudaMemcpyAsync(order, d_order, sizeof(int64_t) * (size_t)h.n_sel, cudaMemcpyDeviceToHost, ss.stream));
+    CLC_CUDA(cudaMemcpyAsync(gain, d_gain, sizeof(double) * (size_t)h.n_sel, cudaMemcpyDeviceToHost, ss.stream));
+  }
+  CLC_CUDA(cudaMemcpyAsync(keep, d_keep, (size_t)n, cudaMemcpyDeviceToHost, ss.stream));
+  CLC_CUDA(cudaStreamSynchronize(ss.stream));
+  *n_selected = h.n_sel;
+  return CLC_OK;
+}
+
+int select_stream_of(clc_problem* p, SelectStream* ss) {
+  if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+  if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+  *ss = SelectStream{p->stream, p->ev0, p->ev1, p->h_done, p->num_sms};
+  return CLC_OK;
+}
+
+// the report of p at pose7 into device rows (b), then the selection on them
+int select_problem(clc_problem* p, const double pose7[7], const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                   double* gain, uint8_t* keep, float* ms_each, int n_runs) {
+  *n_selected = 0;
+  if (p->n_frames == 0) return CLC_OK;
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  double* h_pose = p->pinned->pose;
+  for (int i = 0; i < 7; ++i) h_pose[i] = pose7[i];
+  CLC_CUDA(cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
+  FrameReportBuffers b;
+  rc = frame_report_alloc(p, &b);
+  if (rc == CLC_OK) rc = frame_report_launch(p, b);
+  SelectStream ss{};
+  if (rc == CLC_OK) rc = select_stream_of(p, &ss);
+  for (int i = 0; i < n_runs && rc == CLC_OK; ++i)
+    rc = select_run(ss, b.rows, p->n_frames, desc, n_selected, order, gain, keep, ms_each ? ms_each + i : nullptr);
+  frame_report_free(p, &b);
+  return rc;
+}
+
+// the selection on host rows, uploaded once to `device` (-1: the current one), on a stream of its own
+int select_rows(int device, int64_t n, const clc_frame_row* rows, const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                double* gain, uint8_t* keep) {
+  *n_selected = 0;
+  if (n == 0) return CLC_OK;
+  if (device < 0) CLC_CUDA(cudaGetDevice(&device));
+  CLC_CUDA(cudaSetDevice(device));
+  SelectStream ss{};
+  CLC_CUDA(cudaDeviceGetAttribute(&ss.num_sms, cudaDevAttrMultiProcessorCount, device));
+  struct Owned {
+    SelectStream* s;
+    double* rows = nullptr;
+    ~Owned() {
+      if (rows) cudaFreeAsync(rows, s->stream);
+      if (s->stream) cudaStreamSynchronize(s->stream);
+      if (s->ev0) cudaEventDestroy(s->ev0);
+      if (s->ev1) cudaEventDestroy(s->ev1);
+      if (s->h_flag) cudaFreeHost(s->h_flag);
+      if (s->stream) cudaStreamDestroy(s->stream);
+    }
+  } owned{&ss};
+  CLC_CUDA(cudaStreamCreateWithFlags(&ss.stream, cudaStreamNonBlocking));
+  CLC_CUDA(cudaEventCreate(&ss.ev0));
+  CLC_CUDA(cudaEventCreate(&ss.ev1));
+  CLC_CUDA(cudaMallocHost(&ss.h_flag, sizeof(int)));
+  CLC_CUDA(cudaMallocAsync(&owned.rows, sizeof(clc_frame_row) * (size_t)n, ss.stream));
+  CLC_CUDA(cudaMemcpyAsync(owned.rows, rows, sizeof(clc_frame_row) * (size_t)n, cudaMemcpyHostToDevice, ss.stream));
+  return select_run(ss, owned.rows, n, desc, n_selected, order, gain, keep, nullptr);
+}
+
+}  // namespace
+
+int clc_select_frames(clc_problem* p, const double pose7[7], const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                      double* gain, uint8_t* keep) {
+  if (!p || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
+  int rc = select_check(desc, p->n_frames, n_selected, order, gain, keep);
+  if (rc != CLC_OK) return rc;
+  return select_problem(p, pose7, desc, n_selected, order, gain, keep, nullptr, 1);
+}
+
+int clc_select_frames_rows(int device, int64_t n_frames, const clc_frame_row* rows, const clc_select_desc* desc, int64_t* n_selected,
+                           int64_t* order, double* gain, uint8_t* keep) {
+  if (n_frames < 0 || (n_frames > 0 && !rows)) return fail(CLC_ERR_INVALID, "bad rows");
+  int rc = select_check(desc, n_frames, n_selected, order, gain, keep);
+  if (rc != CLC_OK) return rc;
+  return select_rows(device, n_frames, rows, desc, n_selected, order, gain, keep);
+}
+
+int clc_group_select_frames(clc_group* g, const double pose7[7], const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                            double* gain, uint8_t* keep) {
+  if (!g || g->problems.empty() || !pose7) return fail(CLC_ERR_INVALID, "NULL argument");
+  int rc = select_check(desc, g->n_frames, n_selected, order, gain, keep);
+  if (rc != CLC_OK) return rc;
+  std::vector<clc_frame_row> rows((size_t)g->n_frames);
+  rc = frame_report_all(g->problems.data(), (int)g->problems.size(), pose7, rows.data());
+  if (rc != CLC_OK) return rc;
+  return select_rows(g->problems[0]->device, g->n_frames, rows.data(), desc, n_selected, order, gain, keep);
+}
+
+int clc_bench_select(clc_problem* p, const double pose7[7], const clc_select_desc* desc, int n, float* ms_each, int64_t* n_selected) {
+  if (!p || !pose7 || n < 1 || !ms_each || !n_selected) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  if (p->n_frames == 0) return fail(CLC_ERR_INVALID, "the problem has no frames");
+  const int64_t cap = desc ? std::min(desc->budget, p->n_frames) : 0;
+  std::vector<int64_t> order((size_t)std::max<int64_t>(cap, 1));
+  std::vector<double> gain(order.size());
+  std::vector<uint8_t> keep((size_t)p->n_frames);
+  int rc = select_check(desc, p->n_frames, n_selected, order.data(), gain.data(), keep.data());
+  if (rc != CLC_OK) return rc;
+  return select_problem(p, pose7, desc, n_selected, order.data(), gain.data(), keep.data(), ms_each, n);
 }
 
 int clc_group_solve_lm(clc_group* g, double pose7[7], const clc_lm_options* opt, clc_lm_summary* summary,

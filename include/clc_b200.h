@@ -222,6 +222,42 @@ typedef struct {
  * communicator reports its own frames (its clc_shard_range); no collective. */
 int clc_frame_report(clc_problem* p, const double pose7[7], clc_frame_row* rows);
 
+/* ---- frame selection: the frames that carry the most information about the extrinsic --------------------------------------
+ * Greedy D-optimal selection over the report's per-frame information blocks: which frames to keep (clc_problem_subset takes the
+ * keep mask) instead of a rule on how far the board moved.  Dwell (hundreds of frames that repeat one board pose) adds nothing
+ * new, and a small turn about an axis no kept frame excites yet adds the most.  The rule:
+ *   1. H_f is frame f's H21 of clc_frame_report at pose7, under the problem's loss (the same bytes).  Frame f is usable when its
+ *      21 entries are finite; a frame that is not usable is never picked and never summed.
+ *   2. Only the free coordinates of fixed_mask (clc_lm_options' bits 0-5) count: the principal d x d block, d = 6 - popcount.
+ *   3. T = sum H_f over the usable frames whose state is not 0 (n_T of them).  A free T_kk that is not positive and finite fails
+ *      with CLC_ERR_STATE, clc_last_error naming the coordinate: no frame observes it, so the caller must hold it.  D = diag(T)^-1/2
+ *      and Ht_f = D H_f D (log det does not depend on the units of the coordinates, metres or radians).
+ *   4. A_0 = sum of Ht_f over the usable forced frames + (CLC_SELECT_RIDGE / n_T) I.
+ *   5. Step s: A_s = L L^T; every usable candidate not yet picked has gain_f = log det(I + L^-1 Ht_f L^-T) (in nats), formed from
+ *      the pivots of the Cholesky factorisation of I + C_f (a pivot that is not positive and finite gives -inf).  The largest gain
+ *      is picked, the lowest frame index on a tie.  The selection stops at s = budget, when no candidate is left, or when the best
+ *      gain is <= min_gain; otherwise (f, gain_f) is recorded and A_{s+1} = A_s + Ht_f.
+ * Outputs: *n_selected; order[n_selected] (frame indices in pick order) and gain[n_selected] (caller-sized: min(budget, n_frames)
+ * entries each); keep[n_frames] = 1 for the forced and the picked frames, else 0.  A frame with zero information (an empty frame)
+ * has gain 0 and is never picked at min_gain 0.  Every remaining candidate is evaluated at every step, on the device; two calls
+ * return identical bytes, and the result does not depend on the device or its launch grid.
+ * Rejected before any device work, with CLC_ERR_INVALID: a NULL desc or output, budget < 0, a min_gain that is NaN, negative or
+ * infinite, a state value above 2, a fixed_mask outside [0, 63). */
+#define CLC_SELECT_RIDGE 1e-6 /* A_0's ridge, a millionth of an average frame's scaled diagonal */
+typedef struct {
+  int64_t budget;       /* at most this many picks */
+  double min_gain;      /* stop when the best gain is <= this (nats, finite, >= 0; 0 = stop only at zero information) */
+  int fixed_mask;       /* coordinates left out of the information, as clc_lm_options.fixed_mask */
+  const uint8_t* state; /* [n_frames] 0 = excluded, 1 = candidate, 2 = forced (kept, never picked); NULL = every frame a candidate */
+} clc_select_desc;
+/* The selection on p's report at pose7: the rows stay on the device (one report sweep, then the selection kernels).  A problem
+ * attached to a communicator selects among its own frames. */
+int clc_select_frames(clc_problem* p, const double pose7[7], const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                      double* gain, uint8_t* keep);
+/* The same rule on rows the caller supplies (clc_frame_row, only H21 is read), uploaded once to `device` (-1: the current one). */
+int clc_select_frames_rows(int device, int64_t n_frames, const clc_frame_row* rows, const clc_select_desc* desc, int64_t* n_selected,
+                           int64_t* order, double* gain, uint8_t* keep);
+
 /* Independent extrinsics of runs of consecutive frames (many rigs recorded into one problem, or time windows of one recording),
  * sharing every sweep of the device-resident problem: one pass over the points per evaluation or LM iteration, whatever the
  * number of segments.  Replaces W separate problems (clc_problem_subset of each run) and W clc_eval / clc_information /
@@ -407,6 +443,10 @@ int clc_group_information(clc_group* g, const double pose7[7], double H36[36], d
 int clc_group_closed_form(clc_group* g, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
 /* clc_frame_report of every shard: rows[all frames of the group], in the global frame order */
 int clc_group_frame_report(clc_group* g, const double pose7[7], clc_frame_row* rows);
+/* clc_select_frames for the group: the report rows of every shard in the global frame order (clc_group_frame_report), then
+ * clc_select_frames_rows on the group's first device; order and keep are in the global frame order. */
+int clc_group_select_frames(clc_group* g, const double pose7[7], const clc_select_desc* desc, int64_t* n_selected, int64_t* order,
+                            double* gain, uint8_t* keep);
 /* ---- subsets: solve again without some frames, without sending the points through the host again -----------------------
  * A new problem on src's device holding only the frames with keep[f] == 1 (keep has src's n_frames entries, each 0 or 1), in
  * their original order, built from src's device-resident data: only src's frame offsets come to the host, a gather kernel copies
@@ -470,6 +510,10 @@ int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n,
 /* The same for one time-offset iteration at (pose7, td): each bracket holds the frames' planes and constants, the segment sweep,
  * the fix-up into 36 sums per frame and the two-level reduction (clc_eval_time_offset without the copy to the host). */
 int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int n, int flush_l2, float* ms_each);
+/* clc_select_frames(p, pose7, desc) with the report computed once and the selection run `n` times on its device rows: ms_each[n]
+ * receives the device time of each selection, from its first kernel to the end of its last step (the host polls between step
+ * batches included), and *n_selected the picks of the last run. */
+int clc_bench_select(clc_problem* p, const double pose7[7], const clc_select_desc* desc, int n, float* ms_each, int64_t* n_selected);
 /* The gather of clc_problem_subset(src, keep): `n` times a scratch subset is prepared, its gather kernel is timed alone (CUDA
  * events, after the L2 flush when flush_l2 != 0) and the scratch problem is destroyed.  ms_each[n] receives the device times.
  * Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
