@@ -15,6 +15,7 @@ from .api import (  # noqa: F401
     Group,
     Oberserve,
     Problem,
+    QUANTILES_MAX,
     Selection,
     T_to_pose7,
     comm_unique_id,
@@ -33,4 +34,5 @@ __all__ = [
     "CamLaserCalClosedSolution", "CamLaserCalibration", "LineFittingCeres", "ClcError", "Comm", "Group", "Oberserve", "Problem", "T_to_pose7",
     "comm_unique_id", "default_options", "launch_count", "marshal", "pose7_to_T", "shard_range", "debug_pack", "upload_stats",
     "FRAME_ROW_DTYPE", "frame_influence", "Selection", "select_frames_from_report",
+    "QUANTILES_MAX",
 ]

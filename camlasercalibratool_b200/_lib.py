@@ -194,6 +194,13 @@ SIGNATURES = {
     "clc_group_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.POINTER(_P)]),
     "clc_problem_trim": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(_P)]),
     "clc_group_trim": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(_P)]),
+    "clc_point_residuals": (C.c_int, [_P, c_double_p, C.c_int64, C.c_int64, c_double_p]),
+    "clc_residual_quantiles": (C.c_int, [_P, c_double_p, C.c_int, c_double_p, c_double_p, c_int64_p]),
+    "clc_frame_quantiles": (C.c_int, [_P, c_double_p, C.c_int, c_double_p, c_double_p, c_int64_p]),
+    "clc_group_residual_quantiles": (C.c_int, [_P, c_double_p, C.c_int, c_double_p, c_double_p, c_int64_p]),
+    "clc_group_frame_quantiles": (C.c_int, [_P, c_double_p, C.c_int, c_double_p, c_double_p, c_int64_p]),
+    "clc_bench_quantiles": (C.c_int, [_P, c_double_p, C.c_int, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float),
+                                      C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "clc_default_devices": (C.c_int, [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]),
     "clc_upload_last_stats": (C.c_int, [c_double_p, c_double_p, c_int64_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "clc_problem_destroy": (C.c_int, [_P]),

@@ -273,6 +273,52 @@ def _segments(seg_offsets, poses, n_frames):
     return off, x, W
 
 
+QUANTILES_MAX = 16  # CLC_QUANTILES_MAX
+
+
+def _quantile_args(pose7, q):
+    """pose7 and the quantiles q (a scalar or a 1-D array) -> the float64 arrays of the C ABI and R, checked before any library
+    call: pose7 of 7 finite entries, 1 <= R <= QUANTILES_MAX, every q in [0, 1] (the library checks them too)."""
+    x = np.ascontiguousarray(pose7, dtype=np.float64)
+    if x.shape != (7,) or not np.all(np.isfinite(x)):
+        raise ValueError(f"pose7 must be 7 finite numbers, not {x.shape}")
+    qa = np.asarray(q)
+    if qa.ndim > 1 or not (np.issubdtype(qa.dtype, np.floating) or np.issubdtype(qa.dtype, np.integer)) or qa.dtype == np.bool_:
+        raise ValueError(f"q must be a real scalar or a 1-D real array, not {qa.dtype} of shape {qa.shape}")
+    qa = np.ascontiguousarray(qa.reshape(-1), dtype=np.float64)
+    if not 1 <= qa.size <= QUANTILES_MAX:
+        raise ValueError(f"the number of quantiles must lie in [1, {QUANTILES_MAX}], not {qa.size}")
+    if not np.all((qa >= 0.0) & (qa <= 1.0)):
+        raise ValueError("every q must lie in [0, 1] (NaN is rejected)")
+    return x, qa, qa.size
+
+
+def _residual_quantiles(fn, handle, pose7, q, what):
+    x, qa, R = _quantile_args(pose7, q)
+    values, n_valid = np.empty(R), C.c_int64()
+    _lib.check(fn(handle, _dp(x), R, _dp(qa), _dp(values), C.byref(n_valid)), what)
+    return values, n_valid.value
+
+
+def _frame_quantiles(fn, handle, n_frames, pose7, q, what):
+    x, qa, R = _quantile_args(pose7, q)
+    values, n_valid = np.empty((max(n_frames, 1), R)), np.empty(max(n_frames, 1), dtype=np.int64)
+    _lib.check(fn(handle, _dp(x), R, _dp(qa), _dp(values), _ip(n_valid)), what)
+    return values[:n_frames].copy(), n_valid[:n_frames].copy()
+
+
+def _point_range(first, count, n_points):
+    """(first, count) of point_residuals, checked against [0, n_points]; count None: every point from first on."""
+    for name, v in (("first", first), ("count", count)):
+        if v is not None and (isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer))):
+            raise TypeError(f"{name} must be an integer, not {type(v).__name__}")
+    first = int(first)
+    count = n_points - first if count is None else int(count)
+    if first < 0 or count < 0 or first + count > n_points:
+        raise ValueError(f"the point range [{first}, {first} + {count}) lies outside [0, {n_points}]")
+    return first, count
+
+
 MAX_POSES = 1024
 
 
@@ -555,6 +601,27 @@ class Problem:
                    "clc_information")
         return H, b, chi.value, sv
 
+    def point_residuals(self, pose7, first=0, count=None):
+        """The signed raw distance e of points [first, first + count) to their board at pose7, in point order (clc_point_residuals):
+        the e that frame_report, trim and the quantiles use.  count None: every point from first on.  A range pages through a
+        problem larger than host memory."""
+        x, _, _ = _quantile_args(pose7, 0.0)
+        first, count = _point_range(first, count, self.sizes()[1])
+        e = np.empty(count)
+        _lib.check(self._L.clc_point_residuals(self._h, _dp(x), first, count, _dp(e)), "clc_point_residuals")
+        return e
+
+    def residual_quantiles(self, pose7, q):
+        """Exact quantiles of |e| over every point at pose7 (clc_residual_quantiles): q a scalar or up to QUANTILES_MAX values in
+        [0, 1]; returns (values [R], n_valid).  Quantile q is the k-th smallest valid |e| with k = clamp(ceil(q n) - 1, 0, n - 1)
+        over the n values that are not NaN (q = 0.5: the lower median); NaN when n = 0."""
+        return _residual_quantiles(self._L.clc_residual_quantiles, self._h, pose7, q, "clc_residual_quantiles")
+
+    def frame_quantiles(self, pose7, q):
+        """residual_quantiles within every frame (clc_frame_quantiles): (values [n_frames, R], n_valid [n_frames]).  A robust
+        per-frame trim threshold: 3 * 1.4826 * frame_quantiles(x, 0.5)[0][:, 0]."""
+        return _frame_quantiles(self._L.clc_frame_quantiles, self._h, self.sizes()[0], pose7, q, "clc_frame_quantiles")
+
     def frame_report(self, pose7):
         """Every frame's residual statistics and share of the normal equations at pose7 (clc_frame_report): a numpy record
         array of FRAME_ROW_DTYPE, one row per frame.  Rows sum to eval()'s cost, H (upper triangle) and g, and their chi to
@@ -766,6 +833,16 @@ class Problem:
         _lib.check(self._L.clc_bench_trim(self._h, _dp(pose7), _dp(t), int(n), int(bool(flush_l2)), mark, gather), "clc_bench_trim")
         return np.array(mark[:], dtype=np.float64), np.array(gather[:], dtype=np.float64)
 
+    def bench_quantiles(self, pose7, q, n, flush_l2=True):
+        """Device times of n residual_quantiles(pose7, q) calls, from the first pass to the end of the last, and of n per-frame
+        kernels of frame_quantiles(pose7, q) (clc_bench_quantiles), ms each: returns (problem-wide [n], per-frame [n], passes over
+        the point streams)."""
+        x, qa, R = _quantile_args(pose7, q)
+        ms, fms, passes = (C.c_float * n)(), (C.c_float * n)(), C.c_int()
+        _lib.check(self._L.clc_bench_quantiles(self._h, _dp(x), R, _dp(qa), int(n), int(bool(flush_l2)), ms, fms, C.byref(passes)),
+                   "clc_bench_quantiles")
+        return np.array(ms[:], dtype=np.float64), np.array(fms[:], dtype=np.float64), passes.value
+
 
 class Group:
     """G devices of THIS process solving one problem (clc_group_*): frames sharded by point count, the 28 sums exchanged
@@ -886,6 +963,15 @@ class Group:
     def frame_report(self, pose7):
         """Problem.frame_report over every shard, rows in the global frame order (clc_group_frame_report)."""
         return _frame_report(self._L.clc_group_frame_report, self._h, self.sizes()[1], pose7, "clc_group_frame_report")
+
+    def residual_quantiles(self, pose7, q):
+        """Problem.residual_quantiles over every point of the group (clc_group_residual_quantiles).  A shard's own residuals are
+        problem(i).point_residuals."""
+        return _residual_quantiles(self._L.clc_group_residual_quantiles, self._h, pose7, q, "clc_group_residual_quantiles")
+
+    def frame_quantiles(self, pose7, q):
+        """Problem.frame_quantiles over every shard, rows in the global frame order (clc_group_frame_quantiles)."""
+        return _frame_quantiles(self._L.clc_group_frame_quantiles, self._h, self.sizes()[1], pose7, q, "clc_group_frame_quantiles")
 
     def select_frames(self, pose7, budget, min_gain=0.0, candidates=None, forced=None, fixed=()):
         """Problem.select_frames over every shard (clc_group_select_frames): the frame_report rows in the global frame order,

@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
+#include <limits>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -24,6 +25,7 @@
 #include "clc_kernels.cuh"
 #include "clc_l2_plan.h"
 #include "clc_linefit.cuh"
+#include "clc_quantiles.cuh"
 #include "clc_segments.cuh"
 #include "clc_select.cuh"
 #include "clc_small.cuh"
@@ -3711,6 +3713,267 @@ int clc_group_trim(const clc_group* src, const double pose7[7], const double* ma
   return CLC_OK;
 }
 
+// ---- exact quantiles of the point-to-board distances (clc_quantiles.cuh, clc_quantile_plan.h) --------------------------------
+
+static_assert(clc::kQuantilesMax == CLC_QUANTILES_MAX, "the quantile count of the header");
+
+namespace {
+
+int check_quantiles(const double* pose7, int n_q, const double* q) {
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(pose7[k])) return fail(CLC_ERR_INVALID, "pose7[" + std::to_string(k) + "] is not finite");
+  if (n_q < 1 || n_q > CLC_QUANTILES_MAX)
+    return fail(CLC_ERR_INVALID, "n_q = " + std::to_string(n_q) + " is outside [1, " + std::to_string(CLC_QUANTILES_MAX) + "]");
+  for (int r = 0; r < n_q; ++r)
+    if (!(q[r] >= 0.0 && q[r] <= 1.0)) return fail(CLC_ERR_INVALID, "q[" + std::to_string(r) + "] is NaN or outside [0, 1]");
+  return CLC_OK;
+}
+
+clc::PointStreams point_streams(const clc_problem* p, const double* pose7) {
+  clc::PointStreams s = {};
+  s.x = p->x;
+  s.y = p->y;
+  s.z = p->z_all_zero ? nullptr : p->z;  // a z stream known to be all 0 is not read (as the trim's mark pass)
+  s.plane = p->plane;
+  s.offsets = p->offsets;
+  s.n_frames = p->n_frames;
+  s.n_points = p->n_points;
+  for (int k = 0; k < 7; ++k) s.pose7[k] = pose7[k];
+  return s;
+}
+
+// One shard of a problem-wide selection: its histogram (and the compaction counter after it), its compacted keys.
+struct QuantShard {
+  clc_problem* p = nullptr;
+  int grid = 0;
+  unsigned long long* d_hist = nullptr;  // [2^kQuantileBinsLog2 + 1]
+  uint64_t* d_keys = nullptr;            // [kQuantilesMax * kCompactCap] once compacted
+  int64_t n_keys = 0;
+  std::vector<unsigned long long> h_hist;
+};
+
+int quant_launch(QuantShard& s, const double* pose7, const clc::QSel& sel, int d, int kind) {
+  clc_problem* p = s.p;
+  CLC_CUDA(cudaSetDevice(p->device));
+  const int nb = kind == clc::kPassCompact ? 0 : sel.n_pre << d;
+  CLC_CUDA(cudaMemsetAsync(s.d_hist, 0, sizeof(unsigned long long) * ((size_t)nb + 1), p->stream));
+  clc::QuantPassArgs a = {};
+  a.pts = point_streams(p, pose7);
+  a.keys = s.d_keys;
+  a.n_keys = s.n_keys;
+  a.bits = sel.bits;
+  a.n_pre = sel.n_pre;
+  a.d = d;
+  for (int i = 0; i < sel.n_pre; ++i) a.pre[i] = sel.pre[i];
+  a.hist = s.d_hist;
+  a.out_keys = s.d_keys;
+  a.out_count = s.d_hist + nb;
+  const int64_t work = kind == clc::kPassScratch ? (s.n_keys + clc::kQuantThreads - 1) / clc::kQuantThreads
+                                                 : (p->n_points + clc::kTrimTile - 1) / clc::kTrimTile;
+  const unsigned blocks = (unsigned)std::min<int64_t>(s.grid, work);
+  if (blocks == 0) return CLC_OK;
+  if (kind == clc::kPassPoints) clc::clc_quantile_pass_kernel<clc::kPassPoints><<<blocks, clc::kQuantThreads, 0, p->stream>>>(a);
+  else if (kind == clc::kPassCompact) clc::clc_quantile_pass_kernel<clc::kPassCompact><<<blocks, clc::kQuantThreads, 0, p->stream>>>(a);
+  else clc::clc_quantile_pass_kernel<clc::kPassScratch><<<blocks, clc::kQuantThreads, 0, p->stream>>>(a);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the histogram of the shard's pass added into hist[nb] (compaction: the number of compacted keys into n_keys)
+int quant_collect(QuantShard& s, int nb, int kind, std::vector<uint64_t>* hist) {
+  CLC_CUDA(cudaSetDevice(s.p->device));
+  const int words = kind == clc::kPassCompact ? 1 : nb;
+  s.h_hist.resize((size_t)words);
+  CLC_CUDA(cudaMemcpyAsync(s.h_hist.data(), s.d_hist, sizeof(unsigned long long) * words,
+                           cudaMemcpyDeviceToHost, s.p->stream));
+  CLC_CUDA(cudaStreamSynchronize(s.p->stream));
+  if (kind == clc::kPassCompact) s.n_keys = (int64_t)s.h_hist[0];
+  else
+    for (int b = 0; b < nb; ++b) (*hist)[b] += s.h_hist[b];
+  return CLC_OK;
+}
+
+// The problem-wide selection over the shards ps[0..n): every pass runs on every shard, the histograms are summed on the host.
+// *passes: the passes over the point streams.  ms != nullptr (one shard): the device time from the first pass to the last.
+int quantiles_run(clc_problem* const* ps, int n, const double* pose7, int n_q, const double* q, double* values, int64_t* n_valid,
+                  int* passes, float* ms) {
+  std::vector<QuantShard> shards((size_t)n);
+  clc::QSel sel;
+  clc::qsel_start(&sel, n_q, q);
+  int rc = CLC_OK, n_passes = 0;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  for (int g = 0; g < n && rc == CLC_OK; ++g) {
+    QuantShard& s = shards[g];
+    s.p = ps[g];
+    rc = set_device(s.p);
+    if (rc != CLC_OK) break;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, clc::clc_quantile_pass_kernel<clc::kPassPoints>, clc::kQuantThreads, 0) !=
+            cudaSuccess ||
+        cudaMallocAsync(&s.d_hist, sizeof(unsigned long long) * (((size_t)1 << clc::kQuantileBinsLog2) + 1), s.p->stream) != cudaSuccess)
+      rc = fail(CLC_ERR_CUDA, "quantiles: set-up");
+    s.grid = s.p->num_sms * std::max(per_sm, 1);
+  }
+  if (rc == CLC_OK && ms) {
+    if (cudaEventCreate(&ev[0]) != cudaSuccess || cudaEventCreate(&ev[1]) != cudaSuccess ||
+        cudaEventRecord(ev[0], ps[0]->stream) != cudaSuccess)
+      rc = fail(CLC_ERR_CUDA, "quantiles: events");
+  }
+  bool compacted = false;
+  std::vector<uint64_t> hist;
+  while (rc == CLC_OK && !clc::qsel_done(sel)) {
+    const int d = clc::qsel_digit(sel, clc::kQuantileBinsLog2), nb = sel.n_pre << d;
+    const int kind = compacted ? clc::kPassScratch : clc::kPassPoints;
+    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_launch(shards[g], pose7, sel, d, kind);
+    hist.assign((size_t)nb, 0);
+    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_collect(shards[g], nb, kind, &hist);
+    if (rc != CLC_OK) break;
+    n_passes += compacted ? 0 : 1;
+    clc::qsel_update(&sel, hist.data(), d);
+    if (compacted || clc::qsel_done(sel) || !clc::qsel_fits(sel, clc::kCompactCap)) continue;
+    // every active bucket is small: one more pass over the points copies their keys out, the remaining digits read those
+    for (int g = 0; g < n && rc == CLC_OK; ++g) {
+      QuantShard& s = shards[g];
+      if (cudaSetDevice(s.p->device) != cudaSuccess ||
+          cudaMallocAsync(&s.d_keys, sizeof(uint64_t) * (size_t)sel.n_pre * clc::kCompactCap, s.p->stream) != cudaSuccess)
+        rc = fail(CLC_ERR_CUDA, "quantiles: scratch");
+      if (rc == CLC_OK) rc = quant_launch(s, pose7, sel, 0, clc::kPassCompact);
+    }
+    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_collect(shards[g], 0, clc::kPassCompact, nullptr);
+    n_passes += 1;
+    compacted = true;
+  }
+  if (rc == CLC_OK && ms) {
+    if (cudaEventRecord(ev[1], ps[0]->stream) != cudaSuccess || cudaEventSynchronize(ev[1]) != cudaSuccess ||
+        cudaEventElapsedTime(ms, ev[0], ev[1]) != cudaSuccess)
+      rc = fail(CLC_ERR_CUDA, "quantiles: events");
+  }
+  for (cudaEvent_t e : ev)
+    if (e) cudaEventDestroy(e);
+  for (QuantShard& s : shards)
+    if (s.p && cudaSetDevice(s.p->device) == cudaSuccess) {
+      if (s.d_hist) cudaFreeAsync(s.d_hist, s.p->stream);
+      if (s.d_keys) cudaFreeAsync(s.d_keys, s.p->stream);
+    }
+  if (rc != CLC_OK) return rc;
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  for (int r = 0; r < n_q; ++r) {
+    const uint64_t key = sel.n_valid == 0 ? 0 : clc::qsel_key(sel, r);
+    double v;
+    std::memcpy(&v, &key, sizeof(v));
+    values[r] = sel.n_valid == 0 ? nan : v;
+  }
+  *n_valid = (int64_t)sel.n_valid;
+  if (passes) *passes = n_passes;
+  return CLC_OK;
+}
+
+// The per-frame quantiles of one shard on its stream into the device rows d_values [n_frames * n_q], d_valid [n_frames].
+int frame_quantiles_launch(clc_problem* p, const double* pose7, int n_q, const double* q, double* d_values, int64_t* d_valid) {
+  if (p->n_frames == 0) return CLC_OK;
+  clc::FrameQuantArgs a = {};
+  a.pts = point_streams(p, pose7);
+  a.n_q = n_q;
+  for (int r = 0; r < n_q; ++r) a.q[r] = q[r];
+  a.values = d_values;
+  a.n_valid = d_valid;
+  clc::clc_frame_quantiles_kernel<<<(unsigned)p->n_frames, clc::kQuantThreads, 0, p->stream>>>(a);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+// the per-frame quantiles of the shards ps[0..n), rows in the global frame order (every shard enqueued first, then collected)
+int frame_quantiles_all(clc_problem* const* ps, int n, const double* pose7, int n_q, const double* q, double* values, int64_t* n_valid) {
+  std::vector<double*> d_block((size_t)n, nullptr);
+  int rc = CLC_OK;
+  for (int g = 0; g < n && rc == CLC_OK; ++g) {
+    clc_problem* p = ps[g];
+    if (p->n_frames == 0) continue;
+    rc = set_device(p);
+    if (rc == CLC_OK && cudaMallocAsync(&d_block[g], sizeof(double) * (size_t)p->n_frames * (n_q + 1), p->stream) != cudaSuccess)
+      rc = fail(CLC_ERR_CUDA, "frame quantiles: allocation");
+    if (rc == CLC_OK)
+      rc = frame_quantiles_launch(p, pose7, n_q, q, d_block[g], reinterpret_cast<int64_t*>(d_block[g] + p->n_frames * n_q));
+  }
+  int64_t f0 = 0;
+  for (int g = 0; g < n; ++g) {
+    clc_problem* p = ps[g];
+    if (d_block[g] != nullptr) {
+      cudaSetDevice(p->device);
+      if (rc == CLC_OK) {
+        cudaError_t e = cudaMemcpyAsync(values + f0 * n_q, d_block[g], sizeof(double) * (size_t)p->n_frames * n_q,
+                                        cudaMemcpyDeviceToHost, p->stream);
+        if (e == cudaSuccess)
+          e = cudaMemcpyAsync(n_valid + f0, d_block[g] + p->n_frames * n_q, sizeof(int64_t) * (size_t)p->n_frames,
+                              cudaMemcpyDeviceToHost, p->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
+        if (e != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("frame quantiles: ") + cudaGetErrorString(e));
+      }
+      cudaFreeAsync(d_block[g], p->stream);
+    }
+    f0 += p->n_frames;
+  }
+  return rc;
+}
+
+}  // namespace
+
+int clc_point_residuals(const clc_problem* p, const double pose7[7], int64_t first, int64_t count, double* e) {
+  if (!p || !pose7 || (!e && count > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
+  for (int k = 0; k < 7; ++k)
+    if (!std::isfinite(pose7[k])) return fail(CLC_ERR_INVALID, "pose7[" + std::to_string(k) + "] is not finite");
+  if (first < 0 || count < 0 || first > p->n_points || count > p->n_points - first)
+    return fail(CLC_ERR_INVALID, "the point range [" + std::to_string(first) + ", " + std::to_string(first) + " + " +
+                                     std::to_string(count) + ") is outside [0, " + std::to_string(p->n_points) + "]");
+  if (count == 0) return CLC_OK;
+  int rc = set_device(p);
+  if (rc != CLC_OK) return rc;
+  const int64_t chunk = std::min<int64_t>(count, (int64_t)1 << 24);  // 128 MiB of device staging per copy
+  double* d_out = nullptr;
+  CLC_CUDA(cudaMallocAsync(&d_out, sizeof(double) * chunk, p->stream));
+  const clc::PointStreams s = point_streams(p, pose7);
+  for (int64_t done = 0; done < count && rc == CLC_OK; done += chunk) {
+    const int64_t len = std::min(chunk, count - done);
+    clc::clc_point_residuals_kernel<<<(unsigned)((len + clc::kTrimTile - 1) / clc::kTrimTile), clc::kQuantThreads, 0, p->stream>>>(
+        s, first + done, len, d_out);
+    cudaError_t err = cudaGetLastError();
+    g_launches.fetch_add(1);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(e + done, d_out, sizeof(double) * len, cudaMemcpyDeviceToHost, p->stream);
+    if (err == cudaSuccess) err = cudaStreamSynchronize(p->stream);
+    if (err != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("point residuals: ") + cudaGetErrorString(err));
+  }
+  cudaFreeAsync(d_out, p->stream);
+  return rc;
+}
+
+int clc_residual_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid) {
+  if (!p || !pose7 || !q || !values || !n_valid) return fail(CLC_ERR_INVALID, "NULL argument");
+  const int rc = check_quantiles(pose7, n_q, q);
+  if (rc != CLC_OK) return rc;
+  return quantiles_run(&p, 1, pose7, n_q, q, values, n_valid, nullptr, nullptr);
+}
+
+int clc_frame_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid) {
+  if (!p || !pose7 || !q || ((!values || !n_valid) && p->n_frames > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
+  const int rc = check_quantiles(pose7, n_q, q);
+  if (rc != CLC_OK) return rc;
+  return frame_quantiles_all(&p, 1, pose7, n_q, q, values, n_valid);
+}
+
+int clc_group_residual_quantiles(clc_group* g, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid) {
+  if (!g || !pose7 || !q || !values || !n_valid) return fail(CLC_ERR_INVALID, "NULL argument");
+  const int rc = check_quantiles(pose7, n_q, q);
+  if (rc != CLC_OK) return rc;
+  return quantiles_run(g->problems.data(), (int)g->problems.size(), pose7, n_q, q, values, n_valid, nullptr, nullptr);
+}
+
+int clc_group_frame_quantiles(clc_group* g, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid) {
+  if (!g || !pose7 || !q || ((!values || !n_valid) && g->n_frames > 0)) return fail(CLC_ERR_INVALID, "NULL argument");
+  const int rc = check_quantiles(pose7, n_q, q);
+  if (rc != CLC_OK) return rc;
+  return frame_quantiles_all(g->problems.data(), (int)g->problems.size(), pose7, n_q, q, values, n_valid);
+}
+
 // Devices the reference-facing drop-in uses (its signatures have no device argument): the environment variable
 // CLC_DEVICES = "0,1,2,3" | "all" | unset (the current device).
 int clc_default_devices(int* devices, int cap, int* n) {
@@ -3999,6 +4262,31 @@ int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_ab
     subset_release(shards);
     g_last_error = msg;
   }
+  return rc;
+}
+
+int clc_bench_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, int n, int flush_l2, float* ms_each,
+                        float* frame_ms_each, int* passes) {
+  if (!p || !pose7 || !q || n < 1 || !ms_each || !frame_ms_each || !passes) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  int rc = check_quantiles(pose7, n_q, q);
+  if (rc == CLC_OK) rc = set_device(p);
+  int flush_smem = 0;
+  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
+  std::vector<double> values((size_t)n_q + (size_t)std::max<int64_t>(p->n_frames, 1) * n_q);
+  int64_t n_valid = 0;
+  for (int i = 0; i < n && rc == CLC_OK; ++i) {
+    if (flush_l2) rc = bench_flush(p, i, flush_smem);
+    if (rc == CLC_OK) rc = quantiles_run(&p, 1, pose7, n_q, q, values.data(), &n_valid, passes, &ms_each[i]);
+  }
+  double* d_block = nullptr;
+  if (rc == CLC_OK && cudaMallocAsync(&d_block, sizeof(double) * (size_t)std::max<int64_t>(p->n_frames, 1) * (n_q + 1), p->stream) !=
+                          cudaSuccess)
+    rc = fail(CLC_ERR_CUDA, "bench quantiles: allocation");
+  if (rc == CLC_OK)
+    rc = bench_loop(p, n, flush_l2, flush_smem, frame_ms_each, [&]() {
+      return frame_quantiles_launch(p, pose7, n_q, q, d_block, reinterpret_cast<int64_t*>(d_block + p->n_frames * n_q));
+    });
+  if (d_block) cudaFreeAsync(d_block, p->stream);
   return rc;
 }
 

@@ -486,6 +486,33 @@ int clc_problem_trim(const clc_problem* src, const double pose7[7], const double
  * problem, so shard boundaries move and kept points may cross devices.  They are read over the peer links under the same
  * temporary memory-pool grants as clc_group_subset's. */
 int clc_group_trim(const clc_group* src, const double pose7[7], const double* max_abs_e, clc_group** out);
+/* ---- exact quantiles of the point-to-board distances ----------------------------------------------------------------------
+ * e is the raw point-to-plane distance of a laser point at pose7, computed exactly as the sweep kernel, clc_frame_report and
+ * clc_problem_trim compute it: m = R^T n, c = n.t + d from pose7 and the frame's board plane, e = fma(m0, x, fma(m1, y, fma(m2, z,
+ * c))).  No scale s and no loss enter it, and the edge residuals are not among the values.  The quantiles are taken over |e|
+ * (fabs, so -0.0 counts as +0.0).  A NaN |e| is left out and not counted in n_valid; +inf is valid and sorts last.
+ * Rank rule: with the n valid values sorted ascending, v_0 <= ... <= v_{n-1}, quantile q in [0, 1] is v_k with
+ * k = clamp(ceil(q * n) - 1, 0, n - 1), q * n a double product.  q = 0 is the minimum, q = 1 the maximum, q = 0.5 the lower
+ * median.  With n = 0 the value is NaN.  A result is one element of the multiset of |e|, so it does not depend on the device, the
+ * grid or the order of any atomic: two calls give identical bytes.
+ * A problem attached to a communicator answers for its own points and frames, with no collective (as clc_frame_report).
+ * Rejected with CLC_ERR_INVALID before any device work: a NULL argument, n_q outside [1, CLC_QUANTILES_MAX], a q that is NaN or
+ * outside [0, 1], a pose7 entry that is not finite, a point range outside [0, n_points]. */
+#define CLC_QUANTILES_MAX 16
+/* The signed e of points [first, first + count) of p, in point order, into e[count] (host memory; e may be NULL when count is 0).
+ * A range lets a caller page through a problem larger than host memory. */
+int clc_point_residuals(const clc_problem* p, const double pose7[7], int64_t first, int64_t count, double* e);
+/* The quantiles q[n_q] of |e| over every point of p: values[n_q], *n_valid the number of valid (not NaN) |e|.  A radix select
+ * on the bits of |e|: every requested rank advances in the same passes over the points (about two histogram passes and one
+ * compacting pass on noisy data; at most 7 passes when massive ties, such as e == 0 everywhere, prevent compaction). */
+int clc_residual_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid);
+/* The same rule within every frame of p: values[n_frames * n_q] (row f holds frame f's quantiles in the order of q),
+ * n_valid[n_frames].  One block per frame. */
+int clc_frame_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid);
+/* The same over an in-process group: the problem-wide values over every point of the group, the frame rows in the global frame
+ * order.  Both are identical to those of a single problem holding the group's frames. */
+int clc_group_residual_quantiles(clc_group* g, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid);
+int clc_group_frame_quantiles(clc_group* g, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid);
 /* clc_problem_set_loss on every shard of g (the clc_group_* calls use it; clc_group_subset / clc_group_trim inherit it). */
 int clc_group_set_loss(clc_group* g, int kind, double a);
 /* The device list the reference-facing drop-in uses (its signatures have no device argument): environment variable
@@ -524,6 +551,13 @@ int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2,
  * the passes is in neither.  Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to src until src is destroyed. */
 int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_abs_e, int n, int flush_l2, float* mark_ms,
                    float* gather_ms);
+/* clc_residual_quantiles(p, pose7, n_q, q) `n` times, then clc_frame_quantiles `n` times, each after the L2 flush when flush_l2 != 0.
+ * ms_each[n] receives the device time of every problem-wide call, from its first pass to the end of its last (the host steps
+ * between the passes included); frame_ms_each[n] the device time of every per-frame kernel, not the copy to the host; *passes the
+ * passes over the point streams the problem-wide call made.  Like clc_bench_eval, the flush leaves its 256 MiB buffer attached to p
+ * until p is destroyed. */
+int clc_bench_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, int n, int flush_l2, float* ms_each,
+                        float* frame_ms_each, int* passes);
 /* Algorithmic bytes of one K1 launch on this problem: 24*P + 40*N + 56*edges + 224 (SURVEY.md section 8(d)). */
 int clc_problem_algorithmic_bytes(const clc_problem* p, int64_t* bytes);
 /* Bytes one K1 launch actually streams: the figure above with 16 instead of 24 bytes per point when the planar
