@@ -19,6 +19,7 @@
 #include <limits>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/clc_b200.h"
@@ -335,23 +336,75 @@ void set_creation_loss(clc_problem* p, int use_loss, double cauchy_a) {
 
 using SweepFn = void (*)(clc::ProblemView, clc::SweepArgs);
 
-// the sweep instantiation of a loss kind (clc::LossKind); nullptr for an unknown kind
+// The kernel instantiation of a loss kind (clc::LossKind): f(L) with L a std::integral_constant of the kind; for an unknown kind
+// the value-initialised result (nullptr).
+template <class F>
+auto loss_instance(int loss, F f) -> decltype(f(std::integral_constant<int, clc::kLossNone>())) {
+  switch (loss) {
+    case clc::kLossNone: return f(std::integral_constant<int, clc::kLossNone>());
+    case clc::kLossCauchy: return f(std::integral_constant<int, clc::kLossCauchy>());
+    case clc::kLossHuber: return f(std::integral_constant<int, clc::kLossHuber>());
+    case clc::kLossSoftL1: return f(std::integral_constant<int, clc::kLossSoftL1>());
+    default: return {};
+  }
+}
+
+// the sweep instantiation of a loss kind; nullptr for an unknown kind
 template <int MODE, bool LOOP = false>
 SweepFn sweep_fn(int loss, bool planar) {
-  using namespace clc;
-  switch (loss) {
-    case kLossNone: return planar ? clc_sweep_kernel<kLossNone, MODE, true, LOOP> : clc_sweep_kernel<kLossNone, MODE, false, LOOP>;
-    case kLossCauchy: return planar ? clc_sweep_kernel<kLossCauchy, MODE, true, LOOP> : clc_sweep_kernel<kLossCauchy, MODE, false, LOOP>;
-    case kLossHuber: return planar ? clc_sweep_kernel<kLossHuber, MODE, true, LOOP> : clc_sweep_kernel<kLossHuber, MODE, false, LOOP>;
-    case kLossSoftL1: return planar ? clc_sweep_kernel<kLossSoftL1, MODE, true, LOOP> : clc_sweep_kernel<kLossSoftL1, MODE, false, LOOP>;
-    default: return nullptr;
-  }
+  return loss_instance(loss, [planar](auto L) -> SweepFn {
+    return planar ? clc::clc_sweep_kernel<L.value, MODE, true, LOOP> : clc::clc_sweep_kernel<L.value, MODE, false, LOOP>;
+  });
 }
 
 int set_device(const clc_problem* p) {
   CLC_CUDA(cudaSetDevice(p->device));
   return CLC_OK;
 }
+
+// The owner of one stream-ordered allocation of a call's own scratch: max(n * sizeof(T), 8) bytes on `stream` of `device` (the
+// current device), returned to that device's pool on the same stream when the owner goes.  The free reports nothing, so that the
+// error of a failed call survives its clean-up.  Problem members are not scratch: clc_problem_destroy frees them.
+template <class T>
+class Scratch {
+ public:
+  Scratch() = default;
+  Scratch(Scratch&& o) noexcept : device_(o.device_), stream_(o.stream_), ptr_(o.ptr_) { o.ptr_ = nullptr; }
+  Scratch& operator=(Scratch&& o) noexcept {
+    std::swap(device_, o.device_);
+    std::swap(stream_, o.stream_);
+    std::swap(ptr_, o.ptr_);
+    return *this;
+  }
+  ~Scratch() {
+    if (!ptr_) return;
+    cudaSetDevice(device_);
+    cudaFreeAsync(ptr_, stream_);
+  }
+  cudaError_t alloc(int device, cudaStream_t stream, size_t n) {
+    device_ = device;
+    stream_ = stream;
+    return cudaMallocAsync(reinterpret_cast<void**>(&ptr_), std::max<size_t>(sizeof(T) * n, 8), stream);
+  }
+  cudaError_t alloc(const clc_problem* p, size_t n) { return alloc(p->device, p->stream, n); }
+  T* get() const { return ptr_; }
+
+ private:
+  int device_ = 0;
+  cudaStream_t stream_ = nullptr;
+  T* ptr_ = nullptr;
+};
+
+// A stream of a call's own, synchronised and destroyed when the call ends: declared before the call's Scratch, so that their
+// frees are queued on it first.
+struct CallStream {
+  cudaStream_t s = nullptr;
+  ~CallStream() {
+    if (!s) return;
+    cudaStreamSynchronize(s);
+    cudaStreamDestroy(s);
+  }
+};
 
 // one K1 launch on the problem's stream
 // collective: the sums of this launch are to be all-reduced (in-kernel when the peer path is active)
@@ -361,13 +414,9 @@ using SmallFn = void (*)(clc::ProblemView, clc::LmState*, int, int, const double
 // POSES: the kernel that runs one cluster per pose in one launch (clc_eval_poses, clc_solve_lm_starts)
 template <bool EVAL, bool POSES = false>
 SmallFn small_fn(int loss) {
-  switch (loss) {
-    case clc::kLossNone: return POSES ? clc::clc_small_poses_kernel<clc::kLossNone, EVAL> : clc::clc_small_lm_kernel<clc::kLossNone, EVAL>;
-    case clc::kLossCauchy: return POSES ? clc::clc_small_poses_kernel<clc::kLossCauchy, EVAL> : clc::clc_small_lm_kernel<clc::kLossCauchy, EVAL>;
-    case clc::kLossHuber: return POSES ? clc::clc_small_poses_kernel<clc::kLossHuber, EVAL> : clc::clc_small_lm_kernel<clc::kLossHuber, EVAL>;
-    case clc::kLossSoftL1: return POSES ? clc::clc_small_poses_kernel<clc::kLossSoftL1, EVAL> : clc::clc_small_lm_kernel<clc::kLossSoftL1, EVAL>;
-    default: return nullptr;
-  }
+  return loss_instance(loss, [](auto L) -> SmallFn {
+    return POSES ? clc::clc_small_poses_kernel<L.value, EVAL> : clc::clc_small_lm_kernel<L.value, EVAL>;
+  });
 }
 
 // kModePoses: the tile of running poses a launch walks, and where every pose's constants, rows and slots lie (SweepArgs)
@@ -1089,16 +1138,13 @@ int clc_problem_download(const clc_problem* p, double* frame_pose, int64_t* offs
   if (edge_points && p->n_edges > 0)
     CLC_CUDA(cudaMemcpy(edge_points, p->edge_pt, sizeof(double) * 3 * p->n_edges, cudaMemcpyDeviceToHost));
   if (points && p->n_points > 0) {
-    double* aos = nullptr;
-    CLC_CUDA(cudaMallocAsync(&aos, sizeof(double) * 3 * p->n_points, p->stream));
+    Scratch<double> aos;
+    CLC_CUDA(aos.alloc(p, 3 * (size_t)p->n_points));
     clc::clc_soa_to_aos_kernel<<<(unsigned)((p->n_points + 255) / 256), 256, 0, p->stream>>>(p->x, p->y, p->z, 0,
-                                                                                          p->n_points, aos);
-    g_launches.fetch_add(1);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(points, aos, sizeof(double) * 3 * p->n_points, cudaMemcpyDeviceToHost, p->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-    cudaFreeAsync(aos, p->stream);
-    if (e != cudaSuccess) return fail(CLC_ERR_CUDA, cudaGetErrorString(e));
+                                                                                          p->n_points, aos.get());
+    CLC_LAUNCH_CHECK();
+    CLC_CUDA(cudaMemcpyAsync(points, aos.get(), sizeof(double) * 3 * p->n_points, cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
   }
   return CLC_OK;
 }
@@ -1316,21 +1362,14 @@ static_assert(offsetof(clc_frame_row, n_points) == 8 * clc::kRowN && offsetof(cl
 namespace {
 
 struct FrameReportBuffers {
-  double* rows = nullptr;   // [n_frames * kRowDoubles]
-  double* slots = nullptr;  // [grid * kWarps * 2 * kSlotDoubles]
+  Scratch<double> rows;   // [n_frames * kRowDoubles]
+  Scratch<double> slots;  // [grid * kWarps * 2 * kSlotDoubles]
 };
 
 int frame_report_alloc(clc_problem* p, FrameReportBuffers* b) {
-  const size_t n_slots = (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles;
-  CLC_CUDA(cudaMallocAsync(&b->rows, sizeof(double) * clc::kRowDoubles * (size_t)std::max<int64_t>(p->n_frames, 1), p->stream));
-  CLC_CUDA(cudaMallocAsync(&b->slots, sizeof(double) * n_slots, p->stream));
+  CLC_CUDA(b->rows.alloc(p, clc::kRowDoubles * (size_t)std::max<int64_t>(p->n_frames, 1)));
+  CLC_CUDA(b->slots.alloc(p, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles));
   return CLC_OK;
-}
-
-void frame_report_free(clc_problem* p, FrameReportBuffers* b) {
-  if (b->rows) cudaFreeAsync(b->rows, p->stream);
-  if (b->slots) cudaFreeAsync(b->slots, p->stream);
-  b->rows = b->slots = nullptr;
 }
 
 // the report at the pose in p->pose: the per-frame sweep, then the fix-up of split and empty frames
@@ -1338,17 +1377,12 @@ int frame_report_launch(clc_problem* p, const FrameReportBuffers& b) {
   const int loss = p->loss_kind;
   const bool edges = p->n_edges > 0;
   int rc = launch_sweep(p, clc::kModeFrames, loss, edges, p->pose, nullptr, nullptr, /*collective=*/false, /*pdl=*/false,
-                        /*loop_sweeps=*/1, /*l2_hints=*/false, b.rows, b.slots);
+                        /*loop_sweeps=*/1, /*l2_hints=*/false, b.rows.get(), b.slots.get());
   if (rc != CLC_OK) return rc;
   const int threads = 256;
   const unsigned blocks = (unsigned)((p->n_frames + threads - 1) / threads);
-  const clc::ProblemView v = make_view(p);
-  void (*fixup)(clc::ProblemView, const double*, int, const double*, double*) =
-      loss == clc::kLossCauchy  ? clc::clc_frame_fixup_kernel<clc::kLossCauchy>
-      : loss == clc::kLossHuber ? clc::clc_frame_fixup_kernel<clc::kLossHuber>
-      : loss == clc::kLossSoftL1 ? clc::clc_frame_fixup_kernel<clc::kLossSoftL1>
-                                 : clc::clc_frame_fixup_kernel<clc::kLossNone>;
-  fixup<<<blocks, threads, 0, p->stream>>>(v, p->pose, edges ? 1 : 0, b.slots, b.rows);
+  const auto fixup = loss_instance(loss, [](auto L) { return clc::clc_frame_fixup_kernel<L.value>; });
+  fixup<<<blocks, threads, 0, p->stream>>>(make_view(p), p->pose, edges ? 1 : 0, b.slots.get(), b.rows.get());
   CLC_LAUNCH_CHECK();
   return CLC_OK;
 }
@@ -1356,37 +1390,28 @@ int frame_report_launch(clc_problem* p, const FrameReportBuffers& b) {
 // the reports of the shards ps[0..n) into rows, shard after shard (the global frame order of a group)
 int frame_report_all(clc_problem* const* ps, int n, const double pose7[7], clc_frame_row* rows) {
   std::vector<FrameReportBuffers> bufs((size_t)n);
-  int rc = CLC_OK;
-  for (int g = 0; g < n && rc == CLC_OK; ++g) {  // enqueue on every device first, then collect
+  for (int g = 0; g < n; ++g) {  // enqueue on every device first, then collect
     clc_problem* p = ps[g];
     if (p->n_frames == 0) continue;
-    rc = set_device(p);
-    if (rc != CLC_OK) break;
+    int rc = set_device(p);
+    if (rc != CLC_OK) return rc;
     double* h_pose = p->pinned->pose;
     for (int i = 0; i < 7; ++i) h_pose[i] = pose7[i];
-    if (cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream) != cudaSuccess) {
-      rc = fail(CLC_ERR_CUDA, "pose upload failed");
-      break;
-    }
-    rc = frame_report_alloc(p, &bufs[g]);
-    if (rc == CLC_OK) rc = frame_report_launch(p, bufs[g]);
+    CLC_CUDA(cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
+    if ((rc = frame_report_alloc(p, &bufs[g])) != CLC_OK || (rc = frame_report_launch(p, bufs[g])) != CLC_OK) return rc;
   }
   int64_t first = 0;
   for (int g = 0; g < n; ++g) {
     clc_problem* p = ps[g];
-    if (bufs[g].rows != nullptr) {
-      cudaSetDevice(p->device);
-      if (rc == CLC_OK) {
-        cudaError_t e = cudaMemcpyAsync(rows + first, bufs[g].rows, sizeof(clc_frame_row) * (size_t)p->n_frames,
-                                        cudaMemcpyDeviceToHost, p->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-        if (e != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("frame report: ") + cudaGetErrorString(e));
-      }
-      frame_report_free(p, &bufs[g]);
+    if (p->n_frames > 0) {
+      CLC_CUDA(cudaSetDevice(p->device));
+      CLC_CUDA(cudaMemcpyAsync(rows + first, bufs[g].rows.get(), sizeof(clc_frame_row) * (size_t)p->n_frames, cudaMemcpyDeviceToHost,
+                               p->stream));
+      CLC_CUDA(cudaStreamSynchronize(p->stream));
     }
     first += p->n_frames;
   }
-  return rc;
+  return CLC_OK;
 }
 
 }  // namespace
@@ -1516,6 +1541,45 @@ void copy_trace(const clc_lm_iteration* rows, int n_trace, int trace_cap, clc_lm
   const int n = std::min(std::min(n_trace, clc::kTraceMax), trace_cap);
   for (int i = 0; i < n; ++i) trace[i] = rows[i];
 }
+
+extern "C++" {
+// The results of W batched solves: item w's last accepted point (a terminating candidate is not applied, as clc_solve_lm) into
+// x[(D + 1) w ..], its summary into summaries[w] (summaries may be NULL), its recorded rows (rows + w * trace_cap) into
+// trace + w * trace_cap.
+template <int D>
+void lm_write_results(const clc::LmCoreN<D>* cores, int64_t W, const clc_lm_iteration* rows, int trace_cap, float ms, double* x,
+                      clc_lm_summary* summaries, clc_lm_iteration* trace) {
+  for (int64_t w = 0; w < W; ++w) {
+    for (int i = 0; i < D + 1; ++i) x[(D + 1) * w + i] = cores[w].x[i];
+    if (summaries) summary_from_core(cores[w], ms, &summaries[w]);
+    copy_trace(rows + w * trace_cap, cores[w].n_trace, trace_cap, trace + w * trace_cap);
+  }
+}
+
+// The host side of a batched on-device solve of W items (segments, starts on K1, the time offset) whose buffers the caller has
+// prepared: every item's LM state from its start x[(D + 1) w ..] into d_cores, then iterate(cand, stride) -- one LM iteration of
+// every running item, item w's candidate at cand[w * stride] -- in lm_batches until the device counter *d_running reads 0, and
+// lm_write_results.
+template <int D>
+int lm_solve_items(clc_problem* p, int64_t W, const clc_lm_options& opt, double* x, clc::LmCoreN<D>* d_cores,
+                   const clc_lm_iteration* d_trace, int trace_cap, const int* d_running,
+                   const std::function<int(const double*, int64_t)>& iterate, clc_lm_summary* summaries, clc_lm_iteration* trace) {
+  std::vector<clc::LmCoreN<D>> cores((size_t)W);
+  for (int64_t w = 0; w < W; ++w) clc::lm_init(&cores[(size_t)w], x + (D + 1) * w, opt);
+  // pageable source: the copy has read it when it returns
+  CLC_CUDA(cudaMemcpyAsync(d_cores, cores.data(), sizeof(clc::LmCoreN<D>) * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(d_cores) + offsetof(clc::LmCoreN<D>, cand));
+  const int64_t stride = (int64_t)(sizeof(clc::LmCoreN<D>) / sizeof(double));
+  float ms = 0.f;
+  std::vector<clc_lm_iteration> rows;
+  int rc;
+  if ((rc = lm_batches(p, opt, d_running, [&]() { return iterate(cand, stride); }, &ms)) != CLC_OK ||
+      (rc = lm_read_back(p, d_cores, W, d_trace, trace_cap, cores.data(), &rows)) != CLC_OK)
+    return rc;
+  lm_write_results(cores.data(), W, rows.data(), trace_cap, ms, x, summaries, trace);
+  return CLC_OK;
+}
+}  // extern "C++"
 
 int solve_begin(clc_problem* p, const double pose7[7], const clc_lm_options& opt, SolveCtx* ctx) {
   int rc = set_device(p);
@@ -1734,33 +1798,20 @@ int check_segments(const clc_problem* p, int64_t W, const int64_t* seg_offsets, 
 struct SegmentRun {
   clc_problem* p = nullptr;
   int64_t W = 0, n_chunks = 0;
-  int32_t* frame_seg = nullptr;
-  int64_t* chunk_offsets = nullptr;
-  int64_t* seg_chunks = nullptr;
-  double* consts = nullptr;    // [(n_frames + n_edges) * 4]
-  double* raw = nullptr;       // [n_frames * kSegRawDoubles] the sweep's raw row of every whole frame
-  double* rows = nullptr;      // [n_frames * kNumSums]
-  double* slots = nullptr;     // [grid * kWarps * 2 * kSlotDoubles]
-  double* partials = nullptr;  // [n_chunks * kNumSums]
-  double* poses = nullptr;     // [W * 7] eval / information
-  double* sums = nullptr;      // [W * kNumSums] eval / information
-  clc::LmCore* cores = nullptr;    // [W] solve
-  clc_lm_iteration* trace = nullptr;  // [W * trace_cap] solve with a trace
-  int* counters = nullptr;     // [2] solve: segments still running, all done
-  ~SegmentRun() {
-    if (!p) return;
-    cudaSetDevice(p->device);
-    for (void* b : {(void*)frame_seg, (void*)chunk_offsets, (void*)seg_chunks, (void*)consts, (void*)raw, (void*)rows, (void*)slots,
-                    (void*)partials, (void*)poses, (void*)sums, (void*)cores, (void*)trace, (void*)counters})
-      if (b) cudaFreeAsync(b, p->stream);
-  }
+  Scratch<int32_t> frame_seg;
+  Scratch<int64_t> chunk_offsets;
+  Scratch<int64_t> seg_chunks;
+  Scratch<double> consts;    // [(n_frames + n_edges) * 4]
+  Scratch<double> raw;       // [n_frames * kSegRawDoubles] the sweep's raw row of every whole frame
+  Scratch<double> rows;      // [n_frames * kNumSums]
+  Scratch<double> slots;     // [grid * kWarps * 2 * kSlotDoubles]
+  Scratch<double> partials;  // [n_chunks * kNumSums]
+  Scratch<double> poses;     // [W * (D + 1)] evaluation: the points (eval_points)
+  Scratch<double> sums;      // [W * kLmSums<D>] evaluation: their sums
+  Scratch<clc::LmCore> cores;        // [W] solve
+  Scratch<clc_lm_iteration> trace;   // [W * trace_cap] solve with a trace
+  Scratch<int> counters;             // [2] solve: segments still running, all done
 };
-
-int seg_alloc_bytes(clc_problem* p, void** out, size_t bytes) {
-  CLC_CUDA(cudaMallocAsync(out, std::max<size_t>(bytes, 8), p->stream));
-  return CLC_OK;
-}
-#define seg_alloc(p, out, n) seg_alloc_bytes((p), reinterpret_cast<void**>(out), sizeof(**(out)) * (size_t)(n))
 
 // the plan, the work buffers and the problem's eval pose (which the sweep does not use) on the device; rows and partials are
 // `width` doubles wide (the time-offset calls expand every frame into kTdSums)
@@ -1772,40 +1823,68 @@ int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, Segm
   const clc::SegmentPlan plan = clc::segment_plan(p->n_frames, W, seg_offsets);
   r->n_chunks = (int64_t)plan.chunk_offsets.size() - 1;
   const size_t N = (size_t)p->n_frames;
-  if ((rc = seg_alloc(p, &r->frame_seg, N)) != CLC_OK || (rc = seg_alloc(p, &r->chunk_offsets, plan.chunk_offsets.size())) != CLC_OK ||
-      (rc = seg_alloc(p, &r->seg_chunks, plan.seg_chunks.size())) != CLC_OK ||
-      (rc = seg_alloc(p, &r->consts, (N + (size_t)p->n_edges) * 4)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->raw, N * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->rows, N * width)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->slots, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->partials, (size_t)r->n_chunks * width)) != CLC_OK)
-    return rc;
+  CLC_CUDA(r->frame_seg.alloc(p, N));
+  CLC_CUDA(r->chunk_offsets.alloc(p, plan.chunk_offsets.size()));
+  CLC_CUDA(r->seg_chunks.alloc(p, plan.seg_chunks.size()));
+  CLC_CUDA(r->consts.alloc(p, (N + (size_t)p->n_edges) * 4));
+  CLC_CUDA(r->raw.alloc(p, N * clc::kSegRawDoubles));
+  CLC_CUDA(r->rows.alloc(p, N * width));
+  CLC_CUDA(r->slots.alloc(p, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles));
+  CLC_CUDA(r->partials.alloc(p, (size_t)r->n_chunks * width));
   // pageable sources: each copy has read its source when it returns
-  if (N > 0) CLC_CUDA(cudaMemcpyAsync(r->frame_seg, plan.frame_seg.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice, p->stream));
-  CLC_CUDA(cudaMemcpyAsync(r->chunk_offsets, plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
+  if (N > 0)
+    CLC_CUDA(cudaMemcpyAsync(r->frame_seg.get(), plan.frame_seg.data(), sizeof(int32_t) * N, cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->chunk_offsets.get(), plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
                            cudaMemcpyHostToDevice, p->stream));
-  CLC_CUDA(cudaMemcpyAsync(r->seg_chunks, plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(), cudaMemcpyHostToDevice,
-                           p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->seg_chunks.get(), plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(),
+                           cudaMemcpyHostToDevice, p->stream));
   return CLC_OK;
 }
 
+extern "C++" {
 // Steps 4 and 5 of a segmented iteration over rows of kLmSums<D>: the reduction plan of r into sums ([W * kLmSums<D>]
 // or nullptr) and, with cores, lm_update on every segment that has not terminated (running, done: clc_segment_lm_kernel).
-extern "C++" template <int D>
+template <int D>
 int segments_reduce(const SegmentRun& r, double* sums, clc::LmCoreN<D>* cores, clc_lm_iteration* trace, int trace_cap, int* running,
                     int* done) {
   clc_problem* p = r.p;
   if (r.n_chunks > 0) {
     const unsigned cb = (unsigned)((r.n_chunks + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
     clc::clc_segment_chunk_kernel<clc::kLmSums<D>><<<cb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(
-        r.rows, r.chunk_offsets, r.n_chunks, done, r.partials);
+        r.rows.get(), r.chunk_offsets.get(), r.n_chunks, done, r.partials.get());
     CLC_LAUNCH_CHECK();
   }
   const unsigned sb = (unsigned)((r.W + clc::kSegWarpsPerBlock - 1) / clc::kSegWarpsPerBlock);
-  clc::clc_segment_lm_kernel<D><<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.partials, r.seg_chunks, r.W, sums, cores, trace,
-                                                                                   trace_cap, running, done);
+  clc::clc_segment_lm_kernel<D><<<sb, 32 * clc::kSegWarpsPerBlock, 0, p->stream>>>(r.partials.get(), r.seg_chunks.get(), r.W, sums,
+                                                                                   cores, trace, trace_cap, running, done);
   CLC_LAUNCH_CHECK();
   return CLC_OK;
 }
+
+// The points x [W * (D + 1)] of an evaluation of W items on the device (s->poses), and room for their sums (s->sums).
+template <int D>
+int eval_points(SegmentRun* s, int64_t W, const double* x) {
+  clc_problem* p = s->p;
+  CLC_CUDA(s->poses.alloc(p, (size_t)W * (D + 1)));
+  CLC_CUDA(s->sums.alloc(p, (size_t)W * clc::kLmSums<D>));
+  // pageable source: the copy has read it when it returns
+  CLC_CUDA(cudaMemcpyAsync(s->poses.get(), x, sizeof(double) * (D + 1) * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  return CLC_OK;
+}
+
+// A prepared evaluation of W items (the *_eval_prepare functions): iterate() writes their sums to s.sums, the sums come back to
+// the host, and post(sums of item w, w) runs on every item.
+template <int D, class Post>
+int eval_items(const SegmentRun& s, int64_t W, const std::function<int()>& iterate, Post post) {
+  int rc = iterate();
+  if (rc != CLC_OK) return rc;
+  std::vector<double> sums((size_t)W * clc::kLmSums<D>);
+  CLC_CUDA(cudaMemcpyAsync(sums.data(), s.sums.get(), sizeof(double) * sums.size(), cudaMemcpyDeviceToHost, s.p->stream));
+  CLC_CUDA(cudaStreamSynchronize(s.p->stream));
+  for (int64_t w = 0; w < W; ++w) post(sums.data() + w * clc::kLmSums<D>, w);
+  return CLC_OK;
+}
+}  // extern "C++"
 
 // One shared sweep of every segment: pose s at poses[s * pose_stride] on the device.  sums: [W * kNumSums] or nullptr; cores:
 // the solve's LmCores (lm_update runs on every segment that has not terminated), with its trace, counters and `done` flag.
@@ -1818,40 +1897,31 @@ int segments_iteration(const SegmentRun& r, int loss, bool edges, const double* 
   const int threads = 256;
   if (p->n_frames > 0) {
     const unsigned fb = (unsigned)((p->n_frames + threads - 1) / threads);
-    clc::clc_segment_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.frame_seg, poses, pose_stride, with_edges ? 1 : 0, done,
-                                                                  r.consts);
+    clc::clc_segment_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.frame_seg.get(), poses, pose_stride, with_edges ? 1 : 0, done,
+                                                                  r.consts.get());
     CLC_LAUNCH_CHECK();
     int rc = launch_sweep(p, clc::kModeSegments, loss, with_edges, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
-                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.raw, r.slots, r.consts);
+                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.raw.get(), r.slots.get(), r.consts.get());
     if (rc != CLC_OK) return rc;
-    void (*fixup)(clc::ProblemView, const double*, int, const int*, const double*, const double*, double*) =
-        loss == clc::kLossCauchy  ? clc::clc_segment_fixup_kernel<clc::kLossCauchy>
-        : loss == clc::kLossHuber ? clc::clc_segment_fixup_kernel<clc::kLossHuber>
-        : loss == clc::kLossSoftL1 ? clc::clc_segment_fixup_kernel<clc::kLossSoftL1>
-                                   : clc::clc_segment_fixup_kernel<clc::kLossNone>;
-    fixup<<<fb, threads, 0, p->stream>>>(v, r.consts, with_edges ? 1 : 0, done, r.raw, r.slots, r.rows);
+    const auto fixup = loss_instance(loss, [](auto L) { return clc::clc_segment_fixup_kernel<L.value>; });
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.consts.get(), with_edges ? 1 : 0, done, r.raw.get(), r.slots.get(), r.rows.get());
     CLC_LAUNCH_CHECK();
   }
   return segments_reduce(r, sums, cores, trace, trace_cap, counters, done);
 }
 
-// the per-segment sums of one shared sweep at the poses [W * 7] (which: 0 eval, 1 information -- no loss, no edges)
-int eval_segments_run(clc_problem* p, int64_t W, const int64_t* seg_offsets, const double* poses, int which,
-                      std::vector<double>* sums) {
+// An evaluation of the segments at the poses [W * 7] (which: 0 eval, 1 information -- no loss, no edges): its buffers in r, its
+// one shared sweep in *iterate.
+int segments_eval_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, const double* poses, int which, SegmentRun* r,
+                          std::function<int()>* iterate) {
   int rc = check_segments(p, W, seg_offsets, poses);
   if (rc != CLC_OK) return rc;
-  SegmentRun r;
-  if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK) return rc;
-  if ((rc = seg_alloc(p, &r.poses, (size_t)W * 7)) != CLC_OK || (rc = seg_alloc(p, &r.sums, (size_t)W * clc::kNumSums)) != CLC_OK)
-    return rc;
-  CLC_CUDA(cudaMemcpyAsync(r.poses, poses, sizeof(double) * 7 * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  if ((rc = segments_prepare(p, W, seg_offsets, r)) != CLC_OK || (rc = eval_points<6>(r, W, poses)) != CLC_OK) return rc;
   const int loss = which == 0 ? p->loss_kind : clc::kLossNone;
   const bool edges = which == 0 && p->n_edges > 0;
-  rc = segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
-  if (rc != CLC_OK) return rc;
-  sums->resize((size_t)W * clc::kNumSums);
-  CLC_CUDA(cudaMemcpyAsync(sums->data(), r.sums, sizeof(double) * sums->size(), cudaMemcpyDeviceToHost, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  *iterate = [r, loss, edges]() {
+    return segments_iteration(*r, loss, edges, r->poses.get(), 7, r->sums.get(), nullptr, nullptr, 0, nullptr);
+  };
   return CLC_OK;
 }
 
@@ -1860,23 +1930,25 @@ int eval_segments_run(clc_problem* p, int64_t W, const int64_t* seg_offsets, con
 int clc_eval_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36, double* g6,
                       double* cost) {
   if (!cost) return fail(CLC_ERR_INVALID, "NULL argument");
-  std::vector<double> sums;
-  int rc = eval_segments_run(p, n_segments, seg_offsets, poses, 0, &sums);
+  SegmentRun r;
+  std::function<int()> iterate;
+  const int rc = segments_eval_prepare(p, n_segments, seg_offsets, poses, 0, &r, &iterate);
   if (rc != CLC_OK) return rc;
-  for (int64_t s = 0; s < n_segments; ++s)
-    eval_post(sums.data() + s * clc::kNumSums, H36 ? H36 + 36 * s : nullptr, g6 ? g6 + 6 * s : nullptr, cost + s);
-  return CLC_OK;
+  return eval_items<6>(r, n_segments, iterate, [&](const double* sums, int64_t s) {
+    eval_post(sums, H36 ? H36 + 36 * s : nullptr, g6 ? g6 + 6 * s : nullptr, cost + s);
+  });
 }
 
 int clc_information_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, double* H36,
                              double* b6, double* chi, double* singular_values6, double* V36) {
-  std::vector<double> sums;
-  int rc = eval_segments_run(p, n_segments, seg_offsets, poses, 1, &sums);
+  SegmentRun r;
+  std::function<int()> iterate;
+  const int rc = segments_eval_prepare(p, n_segments, seg_offsets, poses, 1, &r, &iterate);
   if (rc != CLC_OK) return rc;
-  for (int64_t s = 0; s < n_segments; ++s)
-    information_post(sums.data() + s * clc::kNumSums, H36 ? H36 + 36 * s : nullptr, b6 ? b6 + 6 * s : nullptr, chi ? chi + s : nullptr,
+  return eval_items<6>(r, n_segments, iterate, [&](const double* sums, int64_t s) {
+    information_post(sums, H36 ? H36 + 36 * s : nullptr, b6 ? b6 + 6 * s : nullptr, chi ? chi + s : nullptr,
                      singular_values6 ? singular_values6 + 6 * s : nullptr, V36 ? V36 + 36 * s : nullptr);
-  return CLC_OK;
+  });
 }
 
 int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, double* poses, const clc_lm_options* opt_in,
@@ -1890,33 +1962,20 @@ int clc_solve_lm_segments(clc_problem* p, int64_t n_segments, const int64_t* seg
   if ((rc = lm_options(opt_in, &opt)) != CLC_OK) return rc;
   const int64_t W = n_segments;
   SegmentRun r;
-  if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK || (rc = seg_alloc(p, &r.cores, (size_t)W)) != CLC_OK ||
-      (rc = seg_alloc(p, &r.counters, 2)) != CLC_OK)
-    return rc;
-  if (trace_cap > 0 && (rc = seg_alloc(p, &r.trace, (size_t)W * trace_cap)) != CLC_OK) return rc;
-  std::vector<clc::LmCore> cores((size_t)W);
-  for (int64_t s = 0; s < W; ++s) clc::lm_init(&cores[s], poses + 7 * s, opt);
-  CLC_CUDA(cudaMemcpyAsync(r.cores, cores.data(), sizeof(clc::LmCore) * (size_t)W, cudaMemcpyHostToDevice, p->stream));
+  if ((rc = segments_prepare(p, W, seg_offsets, &r)) != CLC_OK) return rc;
+  CLC_CUDA(r.cores.alloc(p, (size_t)W));
+  CLC_CUDA(r.counters.alloc(p, 2));
+  if (trace_cap > 0) CLC_CUDA(r.trace.alloc(p, (size_t)W * trace_cap));
   const int counters0[2] = {(int)W, 0};
-  CLC_CUDA(cudaMemcpyAsync(r.counters, counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r.counters.get(), counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
   const int loss = p->loss_kind;
   const bool edges = p->n_edges > 0;
-  // the candidate pose of segment s: cores[s].cand, sizeof(LmCore) / 8 doubles apart
-  const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.cores) + offsetof(clc::LmCore, cand));
-  const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
-  float ms = 0.f;
-  std::vector<clc_lm_iteration> rows;
-  if ((rc = lm_batches(p, opt, r.counters, [&]() {
-         return segments_iteration(r, loss, edges, cand, stride, nullptr, r.cores, r.trace, trace_cap, r.counters);
-       }, &ms)) != CLC_OK ||
-      (rc = lm_read_back(p, r.cores, W, r.trace, trace_cap, cores.data(), &rows)) != CLC_OK)
-    return rc;
-  for (int64_t s = 0; s < W; ++s) {
-    for (int i = 0; i < 7; ++i) poses[7 * s + i] = cores[s].x[i];  // the last accepted point, as clc_solve_lm
-    summary_from_core(cores[s], ms, &summaries[s]);
-    copy_trace(rows.data() + s * trace_cap, cores[s].n_trace, trace_cap, trace + s * trace_cap);
-  }
-  return CLC_OK;
+  return lm_solve_items<6>(p, W, opt, poses, r.cores.get(), r.trace.get(), trace_cap, r.counters.get(),
+                           [&](const double* cand, int64_t stride) {
+                             return segments_iteration(r, loss, edges, cand, stride, nullptr, r.cores.get(), r.trace.get(), trace_cap,
+                                                       r.counters.get());
+                           },
+                           summaries, trace);
 }
 
 // ---- the camera-laser time offset (clc_time_offset.cuh) ---------------------------------------------------------------
@@ -1946,22 +2005,15 @@ int check_time_offset(const clc_problem* p, const double* pose7, const double* t
 // evaluation, sums: its kTdSums sums), plus n, mdot, cdot of every frame and the solve's LM state.
 struct TimeRun {
   SegmentRun s;
-  double* tframe = nullptr;            // [n_frames * kTdFrameDoubles]
-  clc::LmCoreTd* core = nullptr;       // solve
-  ~TimeRun() {
-    if (!s.p) return;
-    cudaSetDevice(s.p->device);
-    for (void* b : {(void*)tframe, (void*)core})
-      if (b) cudaFreeAsync(b, s.p->stream);
-  }
+  Scratch<double> tframe;       // [n_frames * kTdFrameDoubles]
+  Scratch<clc::LmCoreTd> core;  // solve
 };
 
 int time_prepare(clc_problem* p, TimeRun* r) {
   const int64_t off[2] = {0, p->n_frames};
-  int rc;
-  if ((rc = segments_prepare(p, 1, off, &r->s, clc::kTdSums)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->tframe, (size_t)p->n_frames * clc::kTdFrameDoubles)) != CLC_OK)
-    return rc;
+  const int rc = segments_prepare(p, 1, off, &r->s, clc::kTdSums);
+  if (rc != CLC_OK) return rc;
+  CLC_CUDA(r->tframe.alloc(p, (size_t)p->n_frames * clc::kTdFrameDoubles));
   return CLC_OK;
 }
 
@@ -1977,46 +2029,27 @@ int time_iteration(const TimeRun& r, int loss, const double* pose8, double* sums
   const int threads = 256;
   if (p->n_frames > 0) {
     const unsigned fb = (unsigned)((p->n_frames + threads - 1) / threads);
-    clc::clc_time_consts_kernel<<<fb, threads, 0, p->stream>>>(v, tv, frame_time, pose8, done, r.s.consts, r.tframe);
+    clc::clc_time_consts_kernel<<<fb, threads, 0, p->stream>>>(v, tv, frame_time, pose8, done, r.s.consts.get(), r.tframe.get());
     CLC_LAUNCH_CHECK();
     int rc = launch_sweep(p, clc::kModeSegments, loss, false, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
-                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw, r.s.slots, r.s.consts);
+                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw.get(), r.s.slots.get(), r.s.consts.get());
     if (rc != CLC_OK) return rc;
-    void (*fixup)(clc::ProblemView, const double*, const double*, const int*, const double*, const double*, double*) =
-        loss == clc::kLossCauchy  ? clc::clc_time_fixup_kernel<clc::kLossCauchy>
-        : loss == clc::kLossHuber ? clc::clc_time_fixup_kernel<clc::kLossHuber>
-        : loss == clc::kLossSoftL1 ? clc::clc_time_fixup_kernel<clc::kLossSoftL1>
-                                   : clc::clc_time_fixup_kernel<clc::kLossNone>;
-    fixup<<<fb, threads, 0, p->stream>>>(v, r.s.consts, r.tframe, done, r.s.raw, r.s.slots, r.s.rows);
+    const auto fixup = loss_instance(loss, [](auto L) { return clc::clc_time_fixup_kernel<L.value>; });
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.s.consts.get(), r.tframe.get(), done, r.s.raw.get(), r.s.slots.get(), r.s.rows.get());
     CLC_LAUNCH_CHECK();
   }
   return segments_reduce(r.s, sums, core, trace, trace_cap, counters, done);
 }
 
-// the point (pose7, td) and the sum buffers of an evaluation on the device
-int time_eval_prepare(clc_problem* p, const double* pose7, double td, TimeRun* r) {
-  int rc;
-  if ((rc = time_prepare(p, r)) != CLC_OK || (rc = seg_alloc(p, &r->s.poses, 8)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.sums, clc::kTdSums)) != CLC_OK)
-    return rc;
-  double x8[8];
-  for (int i = 0; i < 7; ++i) x8[i] = pose7[i];
-  x8[7] = td;
-  CLC_CUDA(cudaMemcpyAsync(r->s.poses, x8, sizeof(x8), cudaMemcpyHostToDevice, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));  // x8 is pageable and on this stack frame
-  return CLC_OK;
-}
-
-// the kTdSums sums at (pose7, td) (which: 0 eval with the problem's loss, 1 information -- no loss)
-int time_eval_run(clc_problem* p, const double* pose7, double td, int which, double* sums) {
+// An evaluation at (pose7, td) (which: 0 eval with the problem's loss, 1 information -- no loss): its buffers in r, its one
+// iteration in *iterate.
+int time_eval_prepare(clc_problem* p, const double* pose7, double td, int which, TimeRun* r, std::function<int()>* iterate) {
   int rc = check_time_offset(p, pose7, &td);
   if (rc != CLC_OK) return rc;
-  TimeRun r;
-  if ((rc = time_eval_prepare(p, pose7, td, &r)) != CLC_OK) return rc;
-  rc = time_iteration(r, which == 0 ? p->loss_kind : clc::kLossNone, r.s.poses, r.s.sums, nullptr, nullptr, 0, nullptr);
-  if (rc != CLC_OK) return rc;
-  CLC_CUDA(cudaMemcpyAsync(sums, r.s.sums, sizeof(double) * clc::kTdSums, cudaMemcpyDeviceToHost, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
+  const double x8[8] = {pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6], td};
+  if ((rc = time_prepare(p, r)) != CLC_OK || (rc = eval_points<7>(&r->s, 1, x8)) != CLC_OK) return rc;
+  const int loss = which == 0 ? p->loss_kind : clc::kLossNone;
+  *iterate = [r, loss]() { return time_iteration(*r, loss, r->s.poses.get(), r->s.sums.get(), nullptr, nullptr, 0, nullptr); };
   return CLC_OK;
 }
 
@@ -2071,20 +2104,21 @@ int clc_problem_set_trajectory(clc_problem* p, int64_t n_knots, const double* kn
 }
 
 int clc_eval_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double g7[7], double* cost) {
-  double sums[clc::kTdSums];
-  const int rc = time_eval_run(p, pose7, td, 0, sums);
+  TimeRun r;
+  std::function<int()> iterate;
+  const int rc = time_eval_prepare(p, pose7, td, 0, &r, &iterate);
   if (rc != CLC_OK) return rc;
-  eval_post<7>(sums, H49, g7, cost);
-  return CLC_OK;
+  return eval_items<7>(r.s, 1, iterate, [&](const double* sums, int64_t) { eval_post<7>(sums, H49, g7, cost); });
 }
 
 int clc_information_time_offset(clc_problem* p, const double pose7[7], double td, double H49[49], double b7[7], double* chi,
                                 double singular_values7[7], double V49[49]) {
-  double sums[clc::kTdSums];
-  const int rc = time_eval_run(p, pose7, td, 1, sums);
+  TimeRun r;
+  std::function<int()> iterate;
+  const int rc = time_eval_prepare(p, pose7, td, 1, &r, &iterate);
   if (rc != CLC_OK) return rc;
-  information_post<7>(sums, H49, b7, chi, singular_values7, V49);
-  return CLC_OK;
+  return eval_items<7>(r.s, 1, iterate,
+                       [&](const double* sums, int64_t) { information_post<7>(sums, H49, b7, chi, singular_values7, V49); });
 }
 
 int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const clc_lm_options* opt_in, clc_lm_summary* summary,
@@ -2097,29 +2131,22 @@ int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const 
   clc_lm_options opt;
   if ((rc = lm_options(opt_in, &opt, 7)) != CLC_OK) return rc;
   TimeRun r;
-  if ((rc = time_prepare(p, &r)) != CLC_OK || (rc = seg_alloc(p, &r.core, 1)) != CLC_OK ||
-      (rc = seg_alloc(p, &r.s.counters, 2)) != CLC_OK)
-    return rc;
-  if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, trace_cap)) != CLC_OK) return rc;
-  clc::LmCoreTd core;
-  clc::lm_init_td(&core, pose7, *td, opt);
-  // pageable sources: each copy has read its source when it returns
-  CLC_CUDA(cudaMemcpyAsync(r.core, &core, sizeof(core), cudaMemcpyHostToDevice, p->stream));
+  if ((rc = time_prepare(p, &r)) != CLC_OK) return rc;
+  CLC_CUDA(r.core.alloc(p, 1));
+  CLC_CUDA(r.s.counters.alloc(p, 2));
+  if (trace_cap > 0) CLC_CUDA(r.s.trace.alloc(p, trace_cap));
   const int counters0[2] = {1, 0};
-  CLC_CUDA(cudaMemcpyAsync(r.s.counters, counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r.s.counters.get(), counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
   const int loss = p->loss_kind;
-  const double* cand = r.core->cand;  // (pose7, td) of the next sweep
-  float ms = 0.f;
-  std::vector<clc_lm_iteration> rows;
-  if ((rc = lm_batches(p, opt, r.s.counters, [&]() {
-         return time_iteration(r, loss, cand, nullptr, r.core, r.s.trace, trace_cap, r.s.counters);
-       }, &ms)) != CLC_OK ||
-      (rc = lm_read_back(p, r.core, 1, r.s.trace, trace_cap, &core, &rows)) != CLC_OK)
-    return rc;
-  for (int i = 0; i < 7; ++i) pose7[i] = core.x[i];  // the last accepted point, as clc_solve_lm
-  *td = core.x[7];
-  if (summary) summary_from_core(core, ms, summary);
-  copy_trace(rows.data(), core.n_trace, trace_cap, trace);
+  double x8[8] = {pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6], *td};
+  rc = lm_solve_items<7>(p, 1, opt, x8, r.core.get(), r.s.trace.get(), trace_cap, r.s.counters.get(),
+                         [&](const double* cand, int64_t) {  // cand: (pose7, td) of the next sweep
+                           return time_iteration(r, loss, cand, nullptr, r.core.get(), r.s.trace.get(), trace_cap, r.s.counters.get());
+                         },
+                         summary, trace);
+  if (rc != CLC_OK) return rc;
+  for (int i = 0; i < 7; ++i) pose7[i] = x8[i];
+  *td = x8[7];
   return CLC_OK;
 }
 
@@ -2146,15 +2173,9 @@ int check_poses(const clc_problem* p, int64_t K, const double* poses) {
 struct PoseRun {
   SegmentRun s;
   int64_t K = 0;
-  int* active = nullptr;  // [K] running poses, then [3]: poses still running, all done, number of listed poses
-  int* running() const { return active + K; }
-  int* count() const { return active + K + 2; }
-  ~PoseRun() {
-    if (s.p && active) {
-      cudaSetDevice(s.p->device);
-      cudaFreeAsync(active, s.p->stream);
-    }
-  }
+  Scratch<int> active;  // [K] running poses, then [3]: poses still running, all done, number of listed poses
+  int* running() const { return active.get() + K; }
+  int* count() const { return active.get() + K + 2; }
 };
 
 // the plan, the work buffers and the full list of running poses 0 .. K-1 on the device
@@ -2169,25 +2190,25 @@ int poses_prepare(clc_problem* p, int64_t K, PoseRun* r) {
   const clc::SegmentPlan plan = clc::segment_plan(N * K, K, off.data());
   r->s.n_chunks = (int64_t)plan.chunk_offsets.size() - 1;
   const size_t rows = (size_t)(N * K);
-  if ((rc = seg_alloc(p, &r->s.chunk_offsets, plan.chunk_offsets.size())) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.seg_chunks, plan.seg_chunks.size())) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.consts, (size_t)K * (size_t)(N + p->n_edges) * 4)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.raw, rows * clc::kSegRawDoubles)) != CLC_OK || (rc = seg_alloc(p, &r->s.rows, rows * clc::kNumSums)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.slots, (size_t)K * p->grid * clc::kWarps * 2 * clc::kSlotDoubles)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->s.partials, (size_t)r->s.n_chunks * clc::kNumSums)) != CLC_OK ||
-      (rc = seg_alloc(p, &r->active, (size_t)K + 3)) != CLC_OK)
-    return rc;
-  CLC_CUDA(cudaMemcpyAsync(r->s.chunk_offsets, plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
+  CLC_CUDA(r->s.chunk_offsets.alloc(p, plan.chunk_offsets.size()));
+  CLC_CUDA(r->s.seg_chunks.alloc(p, plan.seg_chunks.size()));
+  CLC_CUDA(r->s.consts.alloc(p, (size_t)K * (size_t)(N + p->n_edges) * 4));
+  CLC_CUDA(r->s.raw.alloc(p, rows * clc::kSegRawDoubles));
+  CLC_CUDA(r->s.rows.alloc(p, rows * clc::kNumSums));
+  CLC_CUDA(r->s.slots.alloc(p, (size_t)K * p->grid * clc::kWarps * 2 * clc::kSlotDoubles));
+  CLC_CUDA(r->s.partials.alloc(p, (size_t)r->s.n_chunks * clc::kNumSums));
+  CLC_CUDA(r->active.alloc(p, (size_t)K + 3));
+  CLC_CUDA(cudaMemcpyAsync(r->s.chunk_offsets.get(), plan.chunk_offsets.data(), sizeof(int64_t) * plan.chunk_offsets.size(),
                            cudaMemcpyHostToDevice, p->stream));
-  CLC_CUDA(cudaMemcpyAsync(r->s.seg_chunks, plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(), cudaMemcpyHostToDevice,
-                           p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->s.seg_chunks.get(), plan.seg_chunks.data(), sizeof(int64_t) * plan.seg_chunks.size(),
+                           cudaMemcpyHostToDevice, p->stream));
   std::vector<int> active((size_t)K + 3);
   for (int64_t k = 0; k < K; ++k) active[(size_t)k] = (int)k;
   active[(size_t)K] = (int)K;  // running
   active[(size_t)K + 1] = 0;   // done
   active[(size_t)K + 2] = (int)K;  // listed
   // pageable sources: each copy has read its source when it returns
-  CLC_CUDA(cudaMemcpyAsync(r->active, active.data(), sizeof(int) * active.size(), cudaMemcpyHostToDevice, p->stream));
+  CLC_CUDA(cudaMemcpyAsync(r->active.get(), active.data(), sizeof(int) * active.size(), cudaMemcpyHostToDevice, p->stream));
   return CLC_OK;
 }
 
@@ -2206,29 +2227,24 @@ int poses_iteration(const PoseRun& r, int loss, bool edges, const double* poses,
   const int64_t slots_stride = (int64_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles;
   if (N > 0) {
     const dim3 fb((unsigned)((N + threads - 1) / threads), (unsigned)K);
-    clc::clc_pose_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.active, r.count(), poses, pose_stride, with_edges ? 1 : 0,
-                                                               r.s.consts, consts_stride);
+    clc::clc_pose_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.active.get(), r.count(), poses, pose_stride, with_edges ? 1 : 0,
+                                                               r.s.consts.get(), consts_stride);
     CLC_LAUNCH_CHECK();
     for (int64_t t0 = 0; t0 < K; t0 += clc::kPoseTile) {
-      const PoseTile tile{r.active, r.count(), (int)t0, consts_stride, raw_stride, slots_stride};
+      const PoseTile tile{r.active.get(), r.count(), (int)t0, consts_stride, raw_stride, slots_stride};
       int rc = launch_sweep(p, clc::kModePoses, loss, with_edges, p->pose, done, nullptr, /*collective=*/false, /*pdl=*/false,
-                            /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw, r.s.slots, r.s.consts, &tile);
+                            /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw.get(), r.s.slots.get(), r.s.consts.get(), &tile);
       if (rc != CLC_OK) return rc;
     }
-    void (*fixup)(clc::ProblemView, const int*, const int*, const double*, int64_t, int, const double*, int64_t, const double*,
-                  int64_t, double*) =
-        loss == clc::kLossCauchy  ? clc::clc_pose_fixup_kernel<clc::kLossCauchy>
-        : loss == clc::kLossHuber ? clc::clc_pose_fixup_kernel<clc::kLossHuber>
-        : loss == clc::kLossSoftL1 ? clc::clc_pose_fixup_kernel<clc::kLossSoftL1>
-                                   : clc::clc_pose_fixup_kernel<clc::kLossNone>;
-    fixup<<<fb, threads, 0, p->stream>>>(v, r.active, r.count(), r.s.consts, consts_stride, with_edges ? 1 : 0, r.s.raw, raw_stride,
-                                         r.s.slots, slots_stride, r.s.rows);
+    const auto fixup = loss_instance(loss, [](auto L) { return clc::clc_pose_fixup_kernel<L.value>; });
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.active.get(), r.count(), r.s.consts.get(), consts_stride, with_edges ? 1 : 0, r.s.raw.get(),
+                                         raw_stride, r.s.slots.get(), slots_stride, r.s.rows.get());
     CLC_LAUNCH_CHECK();
   }
   int rc = segments_reduce(r.s, sums, cores, trace, trace_cap, cores != nullptr ? r.running() : nullptr, done);
   if (rc != CLC_OK) return rc;
   if (cores != nullptr) {
-    clc::clc_pose_compact_kernel<<<1, clc::kPoseCompactThreads, 0, p->stream>>>(cores, (int)K, r.active, r.count());
+    clc::clc_pose_compact_kernel<<<1, clc::kPoseCompactThreads, 0, p->stream>>>(cores, (int)K, r.active.get(), r.count());
     CLC_LAUNCH_CHECK();
   }
   return CLC_OK;
@@ -2252,15 +2268,16 @@ int eval_poses_enqueue(clc_problem* p, int64_t K, const double* d_poses, double*
   return poses_iteration(*r, loss, edges, d_poses, 7, d_sums, nullptr, nullptr, 0);
 }
 
-// the work buffers of clc_eval_poses / clc_bench_poses: the poses and sums on the device, and r on K1 problems
-int eval_poses_prepare(clc_problem* p, int64_t K, const double* poses, PoseRun* r) {
-  int rc = set_device(p);
+// An evaluation at the poses [K * 7] (clc_eval_poses, clc_bench_poses): its buffers in r (the K1 plan on problems K2 does not
+// serve), its one launch in *iterate.
+int eval_poses_prepare(clc_problem* p, int64_t K, const double* poses, PoseRun* r, std::function<int()>* iterate) {
+  int rc = check_poses(p, K, poses);
   if (rc != CLC_OK) return rc;
+  if ((rc = set_device(p)) != CLC_OK) return rc;
   r->s.p = p;
   if (!small_kernel_serves(p, p->n_edges > 0) && (rc = poses_prepare(p, K, r)) != CLC_OK) return rc;
-  if ((rc = seg_alloc(p, &r->s.poses, (size_t)K * 7)) != CLC_OK || (rc = seg_alloc(p, &r->s.sums, (size_t)K * clc::kNumSums)) != CLC_OK)
-    return rc;
-  CLC_CUDA(cudaMemcpyAsync(r->s.poses, poses, sizeof(double) * 7 * (size_t)K, cudaMemcpyHostToDevice, p->stream));
+  if ((rc = eval_points<6>(&r->s, K, poses)) != CLC_OK) return rc;
+  *iterate = [p, K, r]() { return eval_poses_enqueue(p, K, r->s.poses.get(), r->s.sums.get(), r); };
   return CLC_OK;
 }
 
@@ -2268,17 +2285,13 @@ int eval_poses_prepare(clc_problem* p, int64_t K, const double* poses, PoseRun* 
 
 int clc_eval_poses(clc_problem* p, int64_t n_poses, const double* poses, double* H36, double* g6, double* cost) {
   if (!cost) return fail(CLC_ERR_INVALID, "NULL argument");
-  int rc = check_poses(p, n_poses, poses);
-  if (rc != CLC_OK) return rc;
   PoseRun r;
-  if ((rc = eval_poses_prepare(p, n_poses, poses, &r)) != CLC_OK) return rc;
-  if ((rc = eval_poses_enqueue(p, n_poses, r.s.poses, r.s.sums, &r)) != CLC_OK) return rc;
-  std::vector<double> sums((size_t)n_poses * clc::kNumSums);
-  CLC_CUDA(cudaMemcpyAsync(sums.data(), r.s.sums, sizeof(double) * sums.size(), cudaMemcpyDeviceToHost, p->stream));
-  CLC_CUDA(cudaStreamSynchronize(p->stream));
-  for (int64_t k = 0; k < n_poses; ++k)
-    eval_post(sums.data() + k * clc::kNumSums, H36 ? H36 + 36 * k : nullptr, g6 ? g6 + 6 * k : nullptr, cost + k);
-  return CLC_OK;
+  std::function<int()> iterate;
+  const int rc = eval_poses_prepare(p, n_poses, poses, &r, &iterate);
+  if (rc != CLC_OK) return rc;
+  return eval_items<6>(r.s, n_poses, iterate, [&](const double* sums, int64_t k) {
+    eval_post(sums, H36 ? H36 + 36 * k : nullptr, g6 ? g6 + 6 * k : nullptr, cost + k);
+  });
 }
 
 int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const clc_lm_options* opt_in, clc_lm_summary* summaries,
@@ -2294,65 +2307,54 @@ int clc_solve_lm_starts(clc_problem* p, int64_t n_poses, double* poses, const cl
   const int64_t K = n_poses;
   const int loss = p->loss_kind;
   const bool edges = p->n_edges > 0;
-  std::vector<clc::LmCore> cores((size_t)K);
-  std::vector<clc_lm_iteration> rows;  // [K * trace_cap]
-  float ms = 0.f;
   if (p->loop_in_kernel >= 1 && fused_lm_update(p) && small_kernel_serves(p, edges)) {
     // the whole solve of every start in one launch, one cluster per start (the path clc_solve_lm takes for this problem)
     const SmallFn fn = small_poses_fn(loss, false);
     if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     std::vector<clc::LmState> states((size_t)K);
     for (int64_t k = 0; k < K; ++k) clc::lm_init(&states[(size_t)k].core, poses + 7 * k, opt);
-    clc::LmState* d_states = nullptr;
-    if ((rc = seg_alloc(p, &d_states, (size_t)K)) != CLC_OK) return rc;
-    struct Free {
-      clc_problem* p;
-      void* b;
-      ~Free() { cudaFreeAsync(b, p->stream); }
-    } free_states{p, d_states};
+    Scratch<clc::LmState> d_states;
+    CLC_CUDA(d_states.alloc(p, (size_t)K));
     // without a trace only the LmCore at the head of every state travels (the kernel writes the trace rows on the device)
     const size_t moved = trace_cap > 0 ? sizeof(clc::LmState) : sizeof(clc::LmCore);
-    CLC_CUDA(cudaMemcpy2DAsync(d_states, sizeof(clc::LmState), states.data(), sizeof(clc::LmState), moved, (size_t)K,
+    CLC_CUDA(cudaMemcpy2DAsync(d_states.get(), sizeof(clc::LmState), states.data(), sizeof(clc::LmState), moved, (size_t)K,
                                cudaMemcpyHostToDevice, p->stream));
     if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
     if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
     CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
-    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), d_states, lm_max_sweeps(opt),
+    fn<<<(unsigned)(K * clc::kSmallCluster), clc::kSmallThreads, 0, p->stream>>>(make_view(p), d_states.get(), lm_max_sweeps(opt),
                                                                                   edges ? 1 : 0, nullptr, nullptr);
     CLC_LAUNCH_CHECK();
     CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
-    CLC_CUDA(cudaMemcpy2DAsync(states.data(), sizeof(clc::LmState), d_states, sizeof(clc::LmState), moved, (size_t)K,
+    CLC_CUDA(cudaMemcpy2DAsync(states.data(), sizeof(clc::LmState), d_states.get(), sizeof(clc::LmState), moved, (size_t)K,
                                cudaMemcpyDeviceToHost, p->stream));
     CLC_CUDA(cudaStreamSynchronize(p->stream));
+    float ms = 0.f;
     CLC_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
-    rows.resize((size_t)K * trace_cap);
+    std::vector<clc::LmCore> cores((size_t)K);
+    std::vector<clc_lm_iteration> rows((size_t)K * trace_cap);
     for (int64_t k = 0; k < K; ++k) {
       cores[(size_t)k] = states[(size_t)k].core;
       copy_trace(states[(size_t)k].trace, cores[(size_t)k].n_trace, trace_cap, rows.data() + k * trace_cap);
     }
+    lm_write_results(cores.data(), K, rows.data(), trace_cap, ms, poses, summaries, trace);
   } else {
     PoseRun r;
-    if ((rc = poses_prepare(p, K, &r)) != CLC_OK || (rc = seg_alloc(p, &r.s.cores, (size_t)K)) != CLC_OK) return rc;
-    if (trace_cap > 0 && (rc = seg_alloc(p, &r.s.trace, (size_t)K * trace_cap)) != CLC_OK) return rc;
-    for (int64_t k = 0; k < K; ++k) clc::lm_init(&cores[(size_t)k], poses + 7 * k, opt);
-    CLC_CUDA(cudaMemcpyAsync(r.s.cores, cores.data(), sizeof(clc::LmCore) * (size_t)K, cudaMemcpyHostToDevice, p->stream));
-    // the candidate pose of start k: cores[k].cand, sizeof(LmCore) / 8 doubles apart
-    const double* cand = reinterpret_cast<const double*>(reinterpret_cast<const char*>(r.s.cores) + offsetof(clc::LmCore, cand));
-    const int64_t stride = (int64_t)(sizeof(clc::LmCore) / sizeof(double));
-    if ((rc = lm_batches(p, opt, r.running(), [&]() {
-           return poses_iteration(r, loss, edges, cand, stride, nullptr, r.s.cores, r.s.trace, trace_cap);
-         }, &ms)) != CLC_OK ||
-        (rc = lm_read_back(p, r.s.cores, K, r.s.trace, trace_cap, cores.data(), &rows)) != CLC_OK)
-      return rc;
+    if ((rc = poses_prepare(p, K, &r)) != CLC_OK) return rc;
+    CLC_CUDA(r.s.cores.alloc(p, (size_t)K));
+    if (trace_cap > 0) CLC_CUDA(r.s.trace.alloc(p, (size_t)K * trace_cap));
+    rc = lm_solve_items<6>(p, K, opt, poses, r.s.cores.get(), r.s.trace.get(), trace_cap, r.running(),
+                           [&](const double* cand, int64_t stride) {
+                             return poses_iteration(r, loss, edges, cand, stride, nullptr, r.s.cores.get(), r.s.trace.get(), trace_cap);
+                           },
+                           summaries, trace);
+    if (rc != CLC_OK) return rc;
   }
   std::vector<int> term((size_t)K);
   std::vector<double> final_cost((size_t)K);
   for (int64_t k = 0; k < K; ++k) {
-    for (int i = 0; i < 7; ++i) poses[7 * k + i] = cores[(size_t)k].x[i];  // the last accepted point, as clc_solve_lm
-    summary_from_core(cores[(size_t)k], ms, &summaries[k]);
     term[(size_t)k] = summaries[k].termination;
     final_cost[(size_t)k] = summaries[k].final_cost;
-    copy_trace(rows.data() + k * trace_cap, cores[(size_t)k].n_trace, trace_cap, trace + k * trace_cap);
   }
   if (best) *best = clc::best_start(K, term.data(), final_cost.data(), CLC_TERM_FAILURE);
   return CLC_OK;
@@ -2366,23 +2368,17 @@ int clc_problem_line_fit(clc_problem* p, double* lines, int max_num_iterations, 
   if (rc != CLC_OK) return rc;
   const int64_t N = p->n_frames;
   if (N == 0) return CLC_OK;
-  double *d_lines = nullptr, *d_info = nullptr;
-  cudaError_t e = cudaMallocAsync(&d_lines, sizeof(double) * 2 * N, p->stream);
-  if (e == cudaSuccess && info) e = cudaMallocAsync(&d_info, sizeof(double) * 4 * N, p->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_lines, lines, sizeof(double) * 2 * N, cudaMemcpyHostToDevice, p->stream);
-  if (e == cudaSuccess) {
-    const int warps = 8;
-    clc::clc_line_fit_kernel<<<(unsigned)((N + warps - 1) / warps), warps * 32, 0, p->stream>>>(
-        p->x, p->y, p->offsets, N, max_num_iterations, p->cauchy_a, d_lines, d_info);
-    g_launches.fetch_add(1);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(lines, d_lines, sizeof(double) * 2 * N, cudaMemcpyDeviceToHost, p->stream);
-  if (e == cudaSuccess && info) e = cudaMemcpyAsync(info, d_info, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, p->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-  if (d_lines) cudaFreeAsync(d_lines, p->stream);
-  if (d_info) cudaFreeAsync(d_info, p->stream);
-  if (e != cudaSuccess) return fail(CLC_ERR_CUDA, cudaGetErrorString(e));
+  Scratch<double> d_lines, d_info;
+  CLC_CUDA(d_lines.alloc(p, 2 * (size_t)N));
+  if (info) CLC_CUDA(d_info.alloc(p, 4 * (size_t)N));
+  CLC_CUDA(cudaMemcpyAsync(d_lines.get(), lines, sizeof(double) * 2 * N, cudaMemcpyHostToDevice, p->stream));
+  const int warps = 8;
+  clc::clc_line_fit_kernel<<<(unsigned)((N + warps - 1) / warps), warps * 32, 0, p->stream>>>(
+      p->x, p->y, p->offsets, N, max_num_iterations, p->cauchy_a, d_lines.get(), d_info.get());
+  CLC_LAUNCH_CHECK();
+  CLC_CUDA(cudaMemcpyAsync(lines, d_lines.get(), sizeof(double) * 2 * N, cudaMemcpyDeviceToHost, p->stream));
+  if (info) CLC_CUDA(cudaMemcpyAsync(info, d_info.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
   return CLC_OK;
 }
 
@@ -2449,30 +2445,22 @@ int clc_scan_segments(const float* ranges, int64_t n_scans, int64_t n_beams, dou
   if (device < 0) CLC_CUDA(cudaGetDevice(&device));
   if (device >= count) return fail(CLC_ERR_INVALID, "device ordinal out of range");
   CLC_CUDA(cudaSetDevice(device));
-  float* d_r = nullptr;
-  int *d_s = nullptr, *d_e = nullptr;
-  cudaStream_t st;
-  CLC_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  cudaError_t e = cudaMallocAsync(&d_r, sizeof(float) * (size_t)n_scans * (size_t)std::max<int64_t>(n_beams, 1), st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_s, sizeof(int) * n_scans, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_e, sizeof(int) * n_scans, st);
-  if (e == cudaSuccess && n_beams > 0)
-    e = cudaMemcpyAsync(d_r, ranges, sizeof(float) * (size_t)n_scans * (size_t)n_beams, cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) {
-    clc::clc_scan_segments_kernel<<<(unsigned)((n_scans + 127) / 128), 128, 0, st>>>(d_r, n_scans, n_beams, angle_min,
-                                                                                   angle_increment, range_min, d_s, d_e);
-    g_launches.fetch_add(1);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(seg_start, d_s, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(seg_end, d_e, sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (d_r) cudaFreeAsync(d_r, st);
-  if (d_s) cudaFreeAsync(d_s, st);
-  if (d_e) cudaFreeAsync(d_e, st);
-  cudaStreamSynchronize(st);
-  cudaStreamDestroy(st);
-  if (e != cudaSuccess) return fail(CLC_ERR_CUDA, cudaGetErrorString(e));
+  CallStream cs;
+  CLC_CUDA(cudaStreamCreateWithFlags(&cs.s, cudaStreamNonBlocking));
+  const cudaStream_t st = cs.s;
+  Scratch<float> d_r;
+  Scratch<int> d_s, d_e;
+  CLC_CUDA(d_r.alloc(device, st, (size_t)n_scans * (size_t)std::max<int64_t>(n_beams, 1)));
+  CLC_CUDA(d_s.alloc(device, st, (size_t)n_scans));
+  CLC_CUDA(d_e.alloc(device, st, (size_t)n_scans));
+  if (n_beams > 0)
+    CLC_CUDA(cudaMemcpyAsync(d_r.get(), ranges, sizeof(float) * (size_t)n_scans * (size_t)n_beams, cudaMemcpyHostToDevice, st));
+  clc::clc_scan_segments_kernel<<<(unsigned)((n_scans + 127) / 128), 128, 0, st>>>(d_r.get(), n_scans, n_beams, angle_min,
+                                                                                 angle_increment, range_min, d_s.get(), d_e.get());
+  CLC_LAUNCH_CHECK();
+  CLC_CUDA(cudaMemcpyAsync(seg_start, d_s.get(), sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  CLC_CUDA(cudaMemcpyAsync(seg_end, d_e.get(), sizeof(int) * n_scans, cudaMemcpyDeviceToHost, st));
+  CLC_CUDA(cudaStreamSynchronize(st));
   return CLC_OK;
 }
 
@@ -2503,36 +2491,31 @@ int clc_estimate_board_poses(const clc_camera_desc* cam, int64_t n_frames, const
   c.grid_cols = cam->grid_cols;
   c.tag_size = cam->tag_size;
   c.tag_spacing = cam->tag_spacing;
-  int64_t* d_off = nullptr;
-  int *d_ids = nullptr, *d_ok = nullptr;
-  float *d_uv = nullptr, *d_lift = nullptr;
-  double* d_pose = nullptr;
-  cudaStream_t st;
-  CLC_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  CallStream cs;
+  CLC_CUDA(cudaStreamCreateWithFlags(&cs.s, cudaStreamNonBlocking));
+  const cudaStream_t st = cs.s;
   const size_t Dm = (size_t)std::max<int64_t>(D, 1);
-  cudaError_t e = cudaMallocAsync(&d_off, sizeof(int64_t) * (n_frames + 1), st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_ids, sizeof(int) * Dm, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_uv, sizeof(float) * 8 * Dm, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_lift, sizeof(float) * 8 * Dm, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_pose, sizeof(double) * 7 * n_frames, st);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_ok, sizeof(int) * n_frames, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, det_offsets, sizeof(int64_t) * (n_frames + 1), cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess && D > 0) e = cudaMemcpyAsync(d_ids, tag_ids, sizeof(int) * D, cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess && D > 0) e = cudaMemcpyAsync(d_uv, corners_uv, sizeof(float) * 8 * D, cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) {
-    clc::clc_estimate_poses_kernel<<<(unsigned)((n_frames + 63) / 64), 64, 0, st>>>(c, n_frames, d_off, d_ids, d_uv, d_lift, d_pose, d_ok);
-    g_launches.fetch_add(1);
-    e = cudaGetLastError();
+  Scratch<int64_t> d_off;
+  Scratch<int> d_ids, d_ok;
+  Scratch<float> d_uv, d_lift;
+  Scratch<double> d_pose;
+  CLC_CUDA(d_off.alloc(device, st, (size_t)n_frames + 1));
+  CLC_CUDA(d_ids.alloc(device, st, Dm));
+  CLC_CUDA(d_uv.alloc(device, st, 8 * Dm));
+  CLC_CUDA(d_lift.alloc(device, st, 8 * Dm));
+  CLC_CUDA(d_pose.alloc(device, st, 7 * (size_t)n_frames));
+  CLC_CUDA(d_ok.alloc(device, st, (size_t)n_frames));
+  CLC_CUDA(cudaMemcpyAsync(d_off.get(), det_offsets, sizeof(int64_t) * (n_frames + 1), cudaMemcpyHostToDevice, st));
+  if (D > 0) {
+    CLC_CUDA(cudaMemcpyAsync(d_ids.get(), tag_ids, sizeof(int) * D, cudaMemcpyHostToDevice, st));
+    CLC_CUDA(cudaMemcpyAsync(d_uv.get(), corners_uv, sizeof(float) * 8 * D, cudaMemcpyHostToDevice, st));
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(pose_wc, d_pose, sizeof(double) * 7 * n_frames, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(ok, d_ok, sizeof(int) * n_frames, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  void* bufs[] = {d_off, d_ids, d_uv, d_lift, d_pose, d_ok};
-  for (void* b : bufs)
-    if (b) cudaFreeAsync(b, st);
-  cudaStreamSynchronize(st);
-  cudaStreamDestroy(st);
-  if (e != cudaSuccess) return fail(CLC_ERR_CUDA, cudaGetErrorString(e));
+  clc::clc_estimate_poses_kernel<<<(unsigned)((n_frames + 63) / 64), 64, 0, st>>>(c, n_frames, d_off.get(), d_ids.get(), d_uv.get(),
+                                                                                 d_lift.get(), d_pose.get(), d_ok.get());
+  CLC_LAUNCH_CHECK();
+  CLC_CUDA(cudaMemcpyAsync(pose_wc, d_pose.get(), sizeof(double) * 7 * n_frames, cudaMemcpyDeviceToHost, st));
+  CLC_CUDA(cudaMemcpyAsync(ok, d_ok.get(), sizeof(int) * n_frames, cudaMemcpyDeviceToHost, st));
+  CLC_CUDA(cudaStreamSynchronize(st));
   return CLC_OK;
 }
 
@@ -2990,6 +2973,7 @@ int select_check(const clc_select_desc* desc, int64_t n_frames, int64_t* n_selec
 
 // where a selection runs: a stream on a device, two events and pinned host memory for the poll
 struct SelectStream {
+  int device;
   cudaStream_t stream;
   cudaEvent_t ev0, ev1;
   int* h_flag;
@@ -3027,8 +3011,9 @@ int select_run(const SelectStream& ss, const double* d_rows, int64_t n, const cl
   const size_t o_in = off;     off += up8(desc->state ? (size_t)n : 0);
   const size_t o_status = off; off += up8((size_t)n);
   const size_t o_keep = off;   off += up8((size_t)n);
-  char* buf = nullptr;
-  CLC_CUDA(cudaMallocAsync(&buf, off, ss.stream));
+  Scratch<char> scratch;
+  CLC_CUDA(scratch.alloc(ss.device, ss.stream, off));
+  char* buf = scratch.get();
   double* packed = reinterpret_cast<double*>(buf + o_packed);
   double* partials = reinterpret_cast<double*>(buf + o_part);
   clc::SelState* st = reinterpret_cast<clc::SelState*>(buf + o_state);
@@ -3038,11 +3023,6 @@ int select_run(const SelectStream& ss, const double* d_rows, int64_t n, const cl
   uint8_t* d_in = desc->state ? reinterpret_cast<uint8_t*>(buf + o_in) : nullptr;
   uint8_t* status = reinterpret_cast<uint8_t*>(buf + o_status);
   uint8_t* d_keep = reinterpret_cast<uint8_t*>(buf + o_keep);
-  struct FreeOnExit {
-    char* b;
-    cudaStream_t s;
-    ~FreeOnExit() { cudaFreeAsync(b, s); }
-  } free_on_exit{buf, ss.stream};
   if (d_in) CLC_CUDA(cudaMemcpyAsync(d_in, desc->state, (size_t)n, cudaMemcpyHostToDevice, ss.stream));
   CLC_CUDA(cudaEventRecord(ss.ev0, ss.stream));
   clc::clc_select_sum_kernel<<<(unsigned)blocks, clc::kSelThreads, 0, ss.stream>>>(d_rows, clc::kRowDoubles, clc::kRowH, n, d_in, fr,
@@ -3083,7 +3063,7 @@ int select_run(const SelectStream& ss, const double* d_rows, int64_t n, const cl
 int select_stream_of(clc_problem* p, SelectStream* ss) {
   if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
   if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
-  *ss = SelectStream{p->stream, p->ev0, p->ev1, p->h_done, p->num_sms};
+  *ss = SelectStream{p->device, p->stream, p->ev0, p->ev1, p->h_done, p->num_sms};
   return CLC_OK;
 }
 
@@ -3098,14 +3078,13 @@ int select_problem(clc_problem* p, const double pose7[7], const clc_select_desc*
   for (int i = 0; i < 7; ++i) h_pose[i] = pose7[i];
   CLC_CUDA(cudaMemcpyAsync(p->pose, h_pose, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
   FrameReportBuffers b;
-  rc = frame_report_alloc(p, &b);
-  if (rc == CLC_OK) rc = frame_report_launch(p, b);
   SelectStream ss{};
-  if (rc == CLC_OK) rc = select_stream_of(p, &ss);
-  for (int i = 0; i < n_runs && rc == CLC_OK; ++i)
-    rc = select_run(ss, b.rows, p->n_frames, desc, n_selected, order, gain, keep, ms_each ? ms_each + i : nullptr);
-  frame_report_free(p, &b);
-  return rc;
+  if ((rc = frame_report_alloc(p, &b)) != CLC_OK || (rc = frame_report_launch(p, b)) != CLC_OK || (rc = select_stream_of(p, &ss)) != CLC_OK)
+    return rc;
+  for (int i = 0; i < n_runs; ++i)
+    if ((rc = select_run(ss, b.rows.get(), p->n_frames, desc, n_selected, order, gain, keep, ms_each ? ms_each + i : nullptr)) != CLC_OK)
+      return rc;
+  return CLC_OK;
 }
 
 // the selection on host rows, uploaded once to `device` (-1: the current one), on a stream of its own
@@ -3116,12 +3095,11 @@ int select_rows(int device, int64_t n, const clc_frame_row* rows, const clc_sele
   if (device < 0) CLC_CUDA(cudaGetDevice(&device));
   CLC_CUDA(cudaSetDevice(device));
   SelectStream ss{};
+  ss.device = device;
   CLC_CUDA(cudaDeviceGetAttribute(&ss.num_sms, cudaDevAttrMultiProcessorCount, device));
-  struct Owned {
+  struct Owned {  // declared before d_rows: the rows are freed on the stream before it goes
     SelectStream* s;
-    double* rows = nullptr;
     ~Owned() {
-      if (rows) cudaFreeAsync(rows, s->stream);
       if (s->stream) cudaStreamSynchronize(s->stream);
       if (s->ev0) cudaEventDestroy(s->ev0);
       if (s->ev1) cudaEventDestroy(s->ev1);
@@ -3133,9 +3111,10 @@ int select_rows(int device, int64_t n, const clc_frame_row* rows, const clc_sele
   CLC_CUDA(cudaEventCreate(&ss.ev0));
   CLC_CUDA(cudaEventCreate(&ss.ev1));
   CLC_CUDA(cudaMallocHost(&ss.h_flag, sizeof(int)));
-  CLC_CUDA(cudaMallocAsync(&owned.rows, sizeof(clc_frame_row) * (size_t)n, ss.stream));
-  CLC_CUDA(cudaMemcpyAsync(owned.rows, rows, sizeof(clc_frame_row) * (size_t)n, cudaMemcpyHostToDevice, ss.stream));
-  return select_run(ss, owned.rows, n, desc, n_selected, order, gain, keep, nullptr);
+  Scratch<clc_frame_row> d_rows;
+  CLC_CUDA(d_rows.alloc(device, ss.stream, (size_t)n));
+  CLC_CUDA(cudaMemcpyAsync(d_rows.get(), rows, sizeof(clc_frame_row) * (size_t)n, cudaMemcpyHostToDevice, ss.stream));
+  return select_run(ss, reinterpret_cast<const double*>(d_rows.get()), n, desc, n_selected, order, gain, keep, nullptr);
 }
 
 }  // namespace
@@ -3196,23 +3175,19 @@ int check_keep(int64_t n_frames, const uint8_t* keep) {
   return CLC_OK;
 }
 
-// One destination shard of a subset while it is being built: the shell, and the gather's inputs in one device buffer
-// (runs [n_runs * 4] | first run of every tile [n_tiles] | source of every frame [n_frames]).
+// One destination shard of a subset while it is being built: the shell (destroyed with the shard unless finish_shards hands it
+// out), and the gather's inputs in one device buffer (runs [n_runs * 4] | first run of every tile [n_tiles] | source of every
+// frame [n_frames]).
 struct SubsetShard {
   clc_problem* p = nullptr;
-  int64_t* d_work = nullptr;
+  Scratch<int64_t> work;
   clc::SubsetArgs args = {};
   bool gathers_z = false;  // some kept point comes from a source whose z is not known to be all 0
-};
-
-void subset_release(std::vector<SubsetShard>& shards) {
-  for (SubsetShard& s : shards) {
-    if (!s.p) continue;
-    if (s.d_work && cudaSetDevice(s.p->device) == cudaSuccess) cudaFreeAsync(s.d_work, s.p->stream);
-    clc_problem_destroy(s.p);
+  ~SubsetShard() {
+    work = Scratch<int64_t>();  // on the shell's stream, before the shell destroys it
+    clc_problem_destroy(p);
   }
-  shards.clear();
-}
+};
 
 // The shell of a destination shard: sizes, the loss of `src` (kind, a and the line fit's cauchy_a), point arrays with zeroed
 // padding, per-frame arrays, offsets.
@@ -3270,7 +3245,7 @@ int subset_prepare(const std::vector<clc_problem*>& src, const uint8_t* keep, co
   }
   const clc::SubsetPlan plan = clc::subset_plan(S, off_ptr.data(), src_frames.data(), keep, G);
   const bool true_poses = src[0]->frame_pose_true != nullptr;
-  out->assign((size_t)G, SubsetShard());
+  *out = std::vector<SubsetShard>((size_t)G);
   size_t seg = 0;
   for (int d = 0; d < G; ++d) {
     SubsetShard& sh = (*out)[d];
@@ -3298,14 +3273,14 @@ int subset_prepare(const std::vector<clc_problem*>& src, const uint8_t* keep, co
     int rc = subset_shell(&sh.p, devices[d], N, P, offsets.data(), sh.gathers_z, edges, true_poses, src[0]);
     if (rc != CLC_OK) return rc;
     clc_problem* p = sh.p;
-    CLC_CUDA(cudaMallocAsync(&sh.d_work, sizeof(int64_t) * std::max<size_t>(work.size(), 1), p->stream));
+    CLC_CUDA(sh.work.alloc(p, std::max<size_t>(work.size(), 1)));
     if (!work.empty())
-      CLC_CUDA(cudaMemcpyAsync(sh.d_work, work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
+      CLC_CUDA(cudaMemcpyAsync(sh.work.get(), work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
     clc::SubsetArgs& a = sh.args;
     a = base;
-    a.runs = sh.d_work;
-    a.tile_run = sh.d_work + 4 * n_runs;
-    a.frame_src = sh.d_work + 4 * n_runs + n_tiles;
+    a.runs = sh.work.get();
+    a.tile_run = sh.work.get() + 4 * n_runs;
+    a.frame_src = sh.work.get() + 4 * n_runs + n_tiles;
     a.n_runs = n_runs;
     a.n_tiles = n_tiles;
     a.n_frames = N;
@@ -3349,8 +3324,7 @@ int subset_finish(SubsetShard& sh) {
       p->z_block = nullptr;
     }
   }
-  CLC_CUDA(cudaFreeAsync(sh.d_work, p->stream));
-  sh.d_work = nullptr;
+  sh.work = Scratch<int64_t>();
   return finish_create(p);
 }
 
@@ -3437,16 +3411,15 @@ int gather_shards(const std::vector<clc_problem*>& src, const std::vector<int>& 
   return rc;
 }
 
-// After the gathers (rc: how far they got): every destination shard's creation tail, or the release of them all on an error.
+// After the gathers (rc: how far they got): every destination shard's creation tail, then the shells handed out (on an error the
+// shards keep and destroy them).
 int finish_shards(std::vector<SubsetShard>& shards, int rc, std::vector<clc_problem*>* out) {
   for (size_t d = 0; d < shards.size() && rc == CLC_OK; ++d) rc = subset_finish(shards[d]);
-  if (rc != CLC_OK) {
-    const std::string msg = g_last_error;
-    subset_release(shards);
-    g_last_error = msg;
-    return rc;
+  if (rc != CLC_OK) return rc;
+  for (SubsetShard& s : shards) {
+    out->push_back(s.p);
+    s.p = nullptr;
   }
-  for (SubsetShard& s : shards) out->push_back(s.p);
   return CLC_OK;
 }
 
@@ -3516,7 +3489,7 @@ int check_trim(const double* pose7, int64_t n_frames, const double* max_abs_e) {
 // The mark pass of one source shard.  One device buffer: kept points of every tile [n_tiles] and of every frame [n_frames] (next
 // to each other, so that one copy brings both to the host), the thresholds [n_frames], the keep mask [n_tiles * kTrimWords].
 struct TrimMarks {
-  int64_t* d_block = nullptr;
+  Scratch<int64_t> block;
   int64_t n_tiles = 0, n_frames = 0;
   clc::TrimMarkArgs args = {};
   std::vector<int64_t> counts;  // host copy: tile counts, then frame counts
@@ -3527,8 +3500,8 @@ int trim_mark_prepare(clc_problem* q, const double* pose7, const double* max_abs
   m->n_tiles = (q->n_points + clc::kTrimTile - 1) / clc::kTrimTile;
   m->n_frames = q->n_frames;
   const int64_t words = 2 * m->n_frames + m->n_tiles + m->n_tiles * clc::kTrimWords / 2;
-  CLC_CUDA(cudaMallocAsync(&m->d_block, sizeof(int64_t) * std::max<int64_t>(words, 1), q->stream));
-  int64_t* frame_kept = m->d_block + m->n_tiles;
+  CLC_CUDA(m->block.alloc(q, (size_t)std::max<int64_t>(words, 1)));
+  int64_t* frame_kept = m->block.get() + m->n_tiles;
   double* tau = reinterpret_cast<double*>(frame_kept + m->n_frames);
   CLC_CUDA(cudaMemsetAsync(frame_kept, 0, sizeof(int64_t) * m->n_frames, q->stream));
   if (m->n_frames > 0)
@@ -3544,7 +3517,7 @@ int trim_mark_prepare(clc_problem* q, const double* pose7, const double* max_abs
   a.n_points = q->n_points;
   for (int k = 0; k < 7; ++k) a.pose7[k] = pose7[k];
   a.mask = reinterpret_cast<uint32_t*>(tau + m->n_frames);
-  a.tile_kept = m->d_block;
+  a.tile_kept = m->block.get();
   a.frame_kept = reinterpret_cast<unsigned long long*>(frame_kept);
   // pageable host memory: the thresholds have been staged when the copy returns
   return CLC_OK;
@@ -3562,15 +3535,9 @@ int trim_mark_collect(clc_problem* q, TrimMarks* m) {
   CLC_CUDA(cudaSetDevice(q->device));
   m->counts.resize((size_t)(m->n_tiles + m->n_frames));
   if (!m->counts.empty())
-    CLC_CUDA(cudaMemcpyAsync(m->counts.data(), m->d_block, sizeof(int64_t) * m->counts.size(), cudaMemcpyDeviceToHost, q->stream));
+    CLC_CUDA(cudaMemcpyAsync(m->counts.data(), m->block.get(), sizeof(int64_t) * m->counts.size(), cudaMemcpyDeviceToHost, q->stream));
   CLC_CUDA(cudaStreamSynchronize(q->stream));
   return CLC_OK;
-}
-
-void trim_marks_release(const std::vector<clc_problem*>& src, std::vector<TrimMarks>& marks) {
-  for (size_t s = 0; s < marks.size(); ++s)
-    if (marks[s].d_block && cudaSetDevice(src[s]->device) == cudaSuccess) cudaFreeAsync(marks[s].d_block, src[s]->stream);
-  marks.clear();
 }
 
 // Plans the trim from the kept counts and builds the shells of its destination shards, one per entry of `devices`, with the
@@ -3596,7 +3563,7 @@ int trim_prepare(const std::vector<clc_problem*>& src, const std::vector<TrimMar
   }
   const clc::TrimPlan plan = clc::trim_plan(S, src_frames.data(), frame_kept.data(), src_tiles.data(), tile_kept.data(), G);
   const bool true_poses = src[0]->frame_pose_true != nullptr;
-  out->assign((size_t)G, SubsetShard());
+  *out = std::vector<SubsetShard>((size_t)G);
   args->assign((size_t)G, base);
   for (int d = 0; d < G; ++d) {
     SubsetShard& sh = (*out)[d];
@@ -3615,11 +3582,11 @@ int trim_prepare(const std::vector<clc_problem*>& src, const std::vector<TrimMar
     const int64_t t_begin = plan.tile_begin[d], n_tiles = plan.tile_begin[d + 1] - t_begin;
     std::vector<int64_t> work(plan.tile_prefix);
     work.insert(work.end(), plan.first_tile.begin() + t_begin, plan.first_tile.begin() + t_begin + n_tiles);
-    CLC_CUDA(cudaMallocAsync(&sh.d_work, sizeof(int64_t) * work.size(), p->stream));
-    CLC_CUDA(cudaMemcpyAsync(sh.d_work, work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
+    CLC_CUDA(sh.work.alloc(p, work.size()));
+    CLC_CUDA(cudaMemcpyAsync(sh.work.get(), work.data(), sizeof(int64_t) * work.size(), cudaMemcpyHostToDevice, p->stream));
     clc::TrimGatherArgs& a = (*args)[d];
-    a.tile_prefix = sh.d_work;
-    a.first_tile = sh.d_work + plan.tile_prefix.size();
+    a.tile_prefix = sh.work.get();
+    a.first_tile = sh.work.get() + plan.tile_prefix.size();
     a.point_begin = p0;
     a.n_points = P;
     a.n_tiles = n_tiles;
@@ -3668,7 +3635,7 @@ int trim_build(const std::vector<clc_problem*>& src, const double* pose7, const 
       const cudaError_t e = cudaStreamSynchronize(sh.p->stream);
       if (e != cudaSuccess && rc == CLC_OK) rc = fail(CLC_ERR_CUDA, std::string("trim gather: ") + cudaGetErrorString(e));
     }
-  trim_marks_release(src, marks);
+  marks.clear();
   return finish_shards(shards, rc, out);
 }
 
@@ -3746,8 +3713,8 @@ clc::PointStreams point_streams(const clc_problem* p, const double* pose7) {
 struct QuantShard {
   clc_problem* p = nullptr;
   int grid = 0;
-  unsigned long long* d_hist = nullptr;  // [2^kQuantileBinsLog2 + 1]
-  uint64_t* d_keys = nullptr;            // [kQuantilesMax * kCompactCap] once compacted
+  Scratch<unsigned long long> hist;  // [2^kQuantileBinsLog2 + 1]
+  Scratch<uint64_t> keys;            // [kQuantilesMax * kCompactCap] once compacted
   int64_t n_keys = 0;
   std::vector<unsigned long long> h_hist;
 };
@@ -3756,18 +3723,18 @@ int quant_launch(QuantShard& s, const double* pose7, const clc::QSel& sel, int d
   clc_problem* p = s.p;
   CLC_CUDA(cudaSetDevice(p->device));
   const int nb = kind == clc::kPassCompact ? 0 : sel.n_pre << d;
-  CLC_CUDA(cudaMemsetAsync(s.d_hist, 0, sizeof(unsigned long long) * ((size_t)nb + 1), p->stream));
+  CLC_CUDA(cudaMemsetAsync(s.hist.get(), 0, sizeof(unsigned long long) * ((size_t)nb + 1), p->stream));
   clc::QuantPassArgs a = {};
   a.pts = point_streams(p, pose7);
-  a.keys = s.d_keys;
+  a.keys = s.keys.get();
   a.n_keys = s.n_keys;
   a.bits = sel.bits;
   a.n_pre = sel.n_pre;
   a.d = d;
   for (int i = 0; i < sel.n_pre; ++i) a.pre[i] = sel.pre[i];
-  a.hist = s.d_hist;
-  a.out_keys = s.d_keys;
-  a.out_count = s.d_hist + nb;
+  a.hist = s.hist.get();
+  a.out_keys = s.keys.get();
+  a.out_count = s.hist.get() + nb;
   const int64_t work = kind == clc::kPassScratch ? (s.n_keys + clc::kQuantThreads - 1) / clc::kQuantThreads
                                                  : (p->n_points + clc::kTrimTile - 1) / clc::kTrimTile;
   const unsigned blocks = (unsigned)std::min<int64_t>(s.grid, work);
@@ -3784,7 +3751,7 @@ int quant_collect(QuantShard& s, int nb, int kind, std::vector<uint64_t>* hist) 
   CLC_CUDA(cudaSetDevice(s.p->device));
   const int words = kind == clc::kPassCompact ? 1 : nb;
   s.h_hist.resize((size_t)words);
-  CLC_CUDA(cudaMemcpyAsync(s.h_hist.data(), s.d_hist, sizeof(unsigned long long) * words,
+  CLC_CUDA(cudaMemcpyAsync(s.h_hist.data(), s.hist.get(), sizeof(unsigned long long) * words,
                            cudaMemcpyDeviceToHost, s.p->stream));
   CLC_CUDA(cudaStreamSynchronize(s.p->stream));
   if (kind == clc::kPassCompact) s.n_keys = (int64_t)s.h_hist[0];
@@ -3801,61 +3768,52 @@ int quantiles_run(clc_problem* const* ps, int n, const double* pose7, int n_q, c
   clc::QSel sel;
   clc::qsel_start(&sel, n_q, q);
   int rc = CLC_OK, n_passes = 0;
-  cudaEvent_t ev[2] = {nullptr, nullptr};
-  for (int g = 0; g < n && rc == CLC_OK; ++g) {
+  for (int g = 0; g < n; ++g) {
     QuantShard& s = shards[g];
     s.p = ps[g];
-    rc = set_device(s.p);
-    if (rc != CLC_OK) break;
+    if ((rc = set_device(s.p)) != CLC_OK) return rc;
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, clc::clc_quantile_pass_kernel<clc::kPassPoints>, clc::kQuantThreads, 0) !=
-            cudaSuccess ||
-        cudaMallocAsync(&s.d_hist, sizeof(unsigned long long) * (((size_t)1 << clc::kQuantileBinsLog2) + 1), s.p->stream) != cudaSuccess)
-      rc = fail(CLC_ERR_CUDA, "quantiles: set-up");
+    CLC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, clc::clc_quantile_pass_kernel<clc::kPassPoints>, clc::kQuantThreads, 0));
+    CLC_CUDA(s.hist.alloc(s.p, ((size_t)1 << clc::kQuantileBinsLog2) + 1));
     s.grid = s.p->num_sms * std::max(per_sm, 1);
   }
-  if (rc == CLC_OK && ms) {
-    if (cudaEventCreate(&ev[0]) != cudaSuccess || cudaEventCreate(&ev[1]) != cudaSuccess ||
-        cudaEventRecord(ev[0], ps[0]->stream) != cudaSuccess)
-      rc = fail(CLC_ERR_CUDA, "quantiles: events");
+  if (ms) {  // one shard: the problem's events, as the solves'
+    clc_problem* p = ps[0];
+    if (!p->ev0) CLC_CUDA(cudaEventCreate(&p->ev0));
+    if (!p->ev1) CLC_CUDA(cudaEventCreate(&p->ev1));
+    CLC_CUDA(cudaEventRecord(p->ev0, p->stream));
   }
   bool compacted = false;
   std::vector<uint64_t> hist;
-  while (rc == CLC_OK && !clc::qsel_done(sel)) {
+  while (!clc::qsel_done(sel)) {
     const int d = clc::qsel_digit(sel, clc::kQuantileBinsLog2), nb = sel.n_pre << d;
     const int kind = compacted ? clc::kPassScratch : clc::kPassPoints;
-    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_launch(shards[g], pose7, sel, d, kind);
+    for (int g = 0; g < n; ++g)
+      if ((rc = quant_launch(shards[g], pose7, sel, d, kind)) != CLC_OK) return rc;
     hist.assign((size_t)nb, 0);
-    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_collect(shards[g], nb, kind, &hist);
-    if (rc != CLC_OK) break;
+    for (int g = 0; g < n; ++g)
+      if ((rc = quant_collect(shards[g], nb, kind, &hist)) != CLC_OK) return rc;
     n_passes += compacted ? 0 : 1;
     clc::qsel_update(&sel, hist.data(), d);
     if (compacted || clc::qsel_done(sel) || !clc::qsel_fits(sel, clc::kCompactCap)) continue;
     // every active bucket is small: one more pass over the points copies their keys out, the remaining digits read those
-    for (int g = 0; g < n && rc == CLC_OK; ++g) {
+    for (int g = 0; g < n; ++g) {
       QuantShard& s = shards[g];
-      if (cudaSetDevice(s.p->device) != cudaSuccess ||
-          cudaMallocAsync(&s.d_keys, sizeof(uint64_t) * (size_t)sel.n_pre * clc::kCompactCap, s.p->stream) != cudaSuccess)
-        rc = fail(CLC_ERR_CUDA, "quantiles: scratch");
-      if (rc == CLC_OK) rc = quant_launch(s, pose7, sel, 0, clc::kPassCompact);
+      CLC_CUDA(cudaSetDevice(s.p->device));
+      CLC_CUDA(s.keys.alloc(s.p, (size_t)sel.n_pre * clc::kCompactCap));
+      if ((rc = quant_launch(s, pose7, sel, 0, clc::kPassCompact)) != CLC_OK) return rc;
     }
-    for (int g = 0; g < n && rc == CLC_OK; ++g) rc = quant_collect(shards[g], 0, clc::kPassCompact, nullptr);
+    for (int g = 0; g < n; ++g)
+      if ((rc = quant_collect(shards[g], 0, clc::kPassCompact, nullptr)) != CLC_OK) return rc;
     n_passes += 1;
     compacted = true;
   }
-  if (rc == CLC_OK && ms) {
-    if (cudaEventRecord(ev[1], ps[0]->stream) != cudaSuccess || cudaEventSynchronize(ev[1]) != cudaSuccess ||
-        cudaEventElapsedTime(ms, ev[0], ev[1]) != cudaSuccess)
-      rc = fail(CLC_ERR_CUDA, "quantiles: events");
+  if (ms) {
+    clc_problem* p = ps[0];
+    CLC_CUDA(cudaEventRecord(p->ev1, p->stream));
+    CLC_CUDA(cudaEventSynchronize(p->ev1));
+    CLC_CUDA(cudaEventElapsedTime(ms, p->ev0, p->ev1));
   }
-  for (cudaEvent_t e : ev)
-    if (e) cudaEventDestroy(e);
-  for (QuantShard& s : shards)
-    if (s.p && cudaSetDevice(s.p->device) == cudaSuccess) {
-      if (s.d_hist) cudaFreeAsync(s.d_hist, s.p->stream);
-      if (s.d_keys) cudaFreeAsync(s.d_keys, s.p->stream);
-    }
-  if (rc != CLC_OK) return rc;
   const double nan = std::numeric_limits<double>::quiet_NaN();
   for (int r = 0; r < n_q; ++r) {
     const uint64_t key = sel.n_valid == 0 ? 0 : clc::qsel_key(sel, r);
@@ -3884,36 +3842,30 @@ int frame_quantiles_launch(clc_problem* p, const double* pose7, int n_q, const d
 
 // the per-frame quantiles of the shards ps[0..n), rows in the global frame order (every shard enqueued first, then collected)
 int frame_quantiles_all(clc_problem* const* ps, int n, const double* pose7, int n_q, const double* q, double* values, int64_t* n_valid) {
-  std::vector<double*> d_block((size_t)n, nullptr);
-  int rc = CLC_OK;
-  for (int g = 0; g < n && rc == CLC_OK; ++g) {
+  std::vector<Scratch<double>> blocks((size_t)n);
+  for (int g = 0; g < n; ++g) {
     clc_problem* p = ps[g];
     if (p->n_frames == 0) continue;
-    rc = set_device(p);
-    if (rc == CLC_OK && cudaMallocAsync(&d_block[g], sizeof(double) * (size_t)p->n_frames * (n_q + 1), p->stream) != cudaSuccess)
-      rc = fail(CLC_ERR_CUDA, "frame quantiles: allocation");
-    if (rc == CLC_OK)
-      rc = frame_quantiles_launch(p, pose7, n_q, q, d_block[g], reinterpret_cast<int64_t*>(d_block[g] + p->n_frames * n_q));
+    int rc = set_device(p);
+    if (rc != CLC_OK) return rc;
+    CLC_CUDA(blocks[g].alloc(p, (size_t)p->n_frames * (n_q + 1)));
+    double* b = blocks[g].get();
+    if ((rc = frame_quantiles_launch(p, pose7, n_q, q, b, reinterpret_cast<int64_t*>(b + p->n_frames * n_q))) != CLC_OK) return rc;
   }
   int64_t f0 = 0;
   for (int g = 0; g < n; ++g) {
     clc_problem* p = ps[g];
-    if (d_block[g] != nullptr) {
-      cudaSetDevice(p->device);
-      if (rc == CLC_OK) {
-        cudaError_t e = cudaMemcpyAsync(values + f0 * n_q, d_block[g], sizeof(double) * (size_t)p->n_frames * n_q,
-                                        cudaMemcpyDeviceToHost, p->stream);
-        if (e == cudaSuccess)
-          e = cudaMemcpyAsync(n_valid + f0, d_block[g] + p->n_frames * n_q, sizeof(int64_t) * (size_t)p->n_frames,
-                              cudaMemcpyDeviceToHost, p->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-        if (e != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("frame quantiles: ") + cudaGetErrorString(e));
-      }
-      cudaFreeAsync(d_block[g], p->stream);
+    if (p->n_frames > 0) {
+      const double* b = blocks[g].get();
+      CLC_CUDA(cudaSetDevice(p->device));
+      CLC_CUDA(cudaMemcpyAsync(values + f0 * n_q, b, sizeof(double) * (size_t)p->n_frames * n_q, cudaMemcpyDeviceToHost, p->stream));
+      CLC_CUDA(cudaMemcpyAsync(n_valid + f0, b + p->n_frames * n_q, sizeof(int64_t) * (size_t)p->n_frames, cudaMemcpyDeviceToHost,
+                               p->stream));
+      CLC_CUDA(cudaStreamSynchronize(p->stream));
     }
     f0 += p->n_frames;
   }
-  return rc;
+  return CLC_OK;
 }
 
 }  // namespace
@@ -3929,21 +3881,18 @@ int clc_point_residuals(const clc_problem* p, const double pose7[7], int64_t fir
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   const int64_t chunk = std::min<int64_t>(count, (int64_t)1 << 24);  // 128 MiB of device staging per copy
-  double* d_out = nullptr;
-  CLC_CUDA(cudaMallocAsync(&d_out, sizeof(double) * chunk, p->stream));
+  Scratch<double> out;
+  CLC_CUDA(out.alloc(p, (size_t)chunk));
   const clc::PointStreams s = point_streams(p, pose7);
-  for (int64_t done = 0; done < count && rc == CLC_OK; done += chunk) {
+  for (int64_t done = 0; done < count; done += chunk) {
     const int64_t len = std::min(chunk, count - done);
     clc::clc_point_residuals_kernel<<<(unsigned)((len + clc::kTrimTile - 1) / clc::kTrimTile), clc::kQuantThreads, 0, p->stream>>>(
-        s, first + done, len, d_out);
-    cudaError_t err = cudaGetLastError();
-    g_launches.fetch_add(1);
-    if (err == cudaSuccess) err = cudaMemcpyAsync(e + done, d_out, sizeof(double) * len, cudaMemcpyDeviceToHost, p->stream);
-    if (err == cudaSuccess) err = cudaStreamSynchronize(p->stream);
-    if (err != cudaSuccess) rc = fail(CLC_ERR_CUDA, std::string("point residuals: ") + cudaGetErrorString(err));
+        s, first + done, len, out.get());
+    CLC_LAUNCH_CHECK();
+    CLC_CUDA(cudaMemcpyAsync(e + done, out.get(), sizeof(double) * len, cudaMemcpyDeviceToHost, p->stream));
+    CLC_CUDA(cudaStreamSynchronize(p->stream));
   }
-  cudaFreeAsync(d_out, p->stream);
-  return rc;
+  return CLC_OK;
 }
 
 int clc_residual_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, double* values, int64_t* n_valid) {
@@ -4150,49 +4099,38 @@ int clc_bench_eval(clc_problem* p, const double pose7[7], int n, int flush_l2, f
 int clc_bench_segments(clc_problem* p, int64_t n_segments, const int64_t* seg_offsets, const double* poses, int n, int flush_l2,
                        float* ms_each) {
   if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
-  int rc = check_segments(p, n_segments, seg_offsets, poses);
-  if (rc != CLC_OK) return rc;
   SegmentRun r;
-  if ((rc = segments_prepare(p, n_segments, seg_offsets, &r)) != CLC_OK ||
-      (rc = seg_alloc(p, &r.poses, (size_t)n_segments * 7)) != CLC_OK ||
-      (rc = seg_alloc(p, &r.sums, (size_t)n_segments * clc::kNumSums)) != CLC_OK)
-    return rc;
-  CLC_CUDA(cudaMemcpyAsync(r.poses, poses, sizeof(double) * 7 * (size_t)n_segments, cudaMemcpyHostToDevice, p->stream));
+  std::function<int()> iterate;
+  int rc = segments_eval_prepare(p, n_segments, seg_offsets, poses, 0, &r, &iterate);
+  if (rc != CLC_OK) return rc;
   int flush_smem = 0;
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
   if (rc != CLC_OK) return rc;
-  const int loss = p->loss_kind;
-  const bool edges = p->n_edges > 0;
-  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
-    return segments_iteration(r, loss, edges, r.poses, 7, r.sums, nullptr, nullptr, 0, nullptr);
-  });
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, iterate);
 }
 
 int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int n, int flush_l2, float* ms_each) {
   if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
-  int rc = check_time_offset(p, pose7, &td);
-  if (rc != CLC_OK) return rc;
   TimeRun r;
-  if ((rc = time_eval_prepare(p, pose7, td, &r)) != CLC_OK) return rc;
+  std::function<int()> iterate;
+  int rc = time_eval_prepare(p, pose7, td, 0, &r, &iterate);
+  if (rc != CLC_OK) return rc;
   int flush_smem = 0;
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
   if (rc != CLC_OK) return rc;
-  const int loss = p->loss_kind;
-  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() {
-    return time_iteration(r, loss, r.s.poses, r.s.sums, nullptr, nullptr, 0, nullptr);
-  });
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, iterate);
 }
 
 int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n, int flush_l2, float* ms_each) {
   if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
-  int rc = check_poses(p, n_poses, poses);
-  if (rc != CLC_OK) return rc;
   PoseRun r;
-  if ((rc = eval_poses_prepare(p, n_poses, poses, &r)) != CLC_OK) return rc;
+  std::function<int()> iterate;
+  int rc = eval_poses_prepare(p, n_poses, poses, &r, &iterate);
+  if (rc != CLC_OK) return rc;
   int flush_smem = 0;
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
   if (rc != CLC_OK) return rc;
-  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return eval_poses_enqueue(p, n_poses, r.s.poses, r.s.sums, &r); });
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, iterate);
 }
 
 int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flush_l2, float* ms_each) {
@@ -4205,10 +4143,8 @@ int clc_bench_frame_report(clc_problem* p, const double pose7[7], int n, int flu
   if (rc != CLC_OK) return rc;
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
   FrameReportBuffers b;
-  rc = frame_report_alloc(p, &b);
-  if (rc == CLC_OK) rc = bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return frame_report_launch(p, b); });
-  frame_report_free(p, &b);
-  return rc;
+  if ((rc = frame_report_alloc(p, &b)) != CLC_OK) return rc;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, [&]() { return frame_report_launch(p, b); });
 }
 
 int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2, float* ms_each) {
@@ -4216,22 +4152,18 @@ int clc_bench_subset(clc_problem* src, const uint8_t* keep, int n, int flush_l2,
   int rc = check_keep(src->n_frames, keep);
   if (rc != CLC_OK) return rc;
   clc_problem* p = src;
-  rc = set_device(p);
   int flush_smem = 0;
-  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
-  for (int i = 0; i < n && rc == CLC_OK; ++i) {
+  if ((rc = set_device(p)) != CLC_OK || (rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem)) != CLC_OK) return rc;
+  for (int i = 0; i < n; ++i) {
     // a fresh scratch problem every time; its gather runs on the source's stream, behind the source's L2 flush
     std::vector<SubsetShard> shards;
-    rc = subset_prepare({p}, keep, {p->device}, &shards);
-    if (rc == CLC_OK) rc = shards[0].p->stream && cudaStreamSynchronize(shards[0].p->stream) == cudaSuccess
-                                ? CLC_OK : fail(CLC_ERR_CUDA, "scratch problem");
-    if (rc == CLC_OK) rc = set_device(p);
-    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &ms_each[i], [&]() { return subset_launch(shards[0], p->stream); });
-    const std::string msg = g_last_error;
-    subset_release(shards);
-    g_last_error = msg;
+    if ((rc = subset_prepare({p}, keep, {p->device}, &shards)) != CLC_OK) return rc;
+    CLC_CUDA(cudaStreamSynchronize(shards[0].p->stream));
+    if ((rc = set_device(p)) != CLC_OK) return rc;
+    rc = bench_loop(p, 1, flush_l2, flush_smem, &ms_each[i], [&]() { return subset_launch(shards[0], p->stream); });
+    if (rc != CLC_OK) return rc;
   }
-  return rc;
+  return CLC_OK;
 }
 
 int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_abs_e, int n, int flush_l2, float* mark_ms,
@@ -4240,54 +4172,44 @@ int clc_bench_trim(clc_problem* src, const double pose7[7], const double* max_ab
   int rc = check_trim(pose7, src->n_frames, max_abs_e);
   if (rc != CLC_OK) return rc;
   clc_problem* p = src;
-  rc = set_device(p);
   int flush_smem = 0;
-  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
-  for (int i = 0; i < n && rc == CLC_OK; ++i) {
-    // a fresh mark and scratch problem every time; both passes run on the source's stream, each behind its own L2 flush
-    std::vector<TrimMarks> marks(1);
+  if ((rc = set_device(p)) != CLC_OK || (rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem)) != CLC_OK) return rc;
+  for (int i = 0; i < n; ++i) {
+    // a fresh mark and scratch problem every time; both passes run on the source's stream, each behind its own L2 flush.  The
+    // masks and the scratch problem go after bench_loop has synchronised the source's stream: the gather is done with them.
     std::vector<SubsetShard> shards;
+    std::vector<TrimMarks> marks(1);
     std::vector<clc::TrimGatherArgs> args;
-    rc = trim_mark_prepare(p, pose7, max_abs_e, &marks[0]);
-    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &mark_ms[i], [&]() { return trim_mark_launch(marks[0], p->stream); });
-    if (rc == CLC_OK) rc = trim_mark_collect(p, &marks[0]);
-    if (rc == CLC_OK) rc = trim_prepare({p}, marks, {p->device}, &shards, &args);
-    if (rc == CLC_OK) rc = shards[0].p->stream && cudaStreamSynchronize(shards[0].p->stream) == cudaSuccess
-                                ? CLC_OK : fail(CLC_ERR_CUDA, "scratch problem");
-    if (rc == CLC_OK) rc = set_device(p);
-    if (rc == CLC_OK) rc = bench_loop(p, 1, flush_l2, flush_smem, &gather_ms[i], [&]() { return trim_launch(args[0], p->stream); });
-    const std::string msg = g_last_error;
-    if (set_device(p) == CLC_OK) cudaStreamSynchronize(p->stream);
-    trim_marks_release({p}, marks);
-    subset_release(shards);
-    g_last_error = msg;
+    if ((rc = trim_mark_prepare(p, pose7, max_abs_e, &marks[0])) != CLC_OK ||
+        (rc = bench_loop(p, 1, flush_l2, flush_smem, &mark_ms[i], [&]() { return trim_mark_launch(marks[0], p->stream); })) != CLC_OK ||
+        (rc = trim_mark_collect(p, &marks[0])) != CLC_OK || (rc = trim_prepare({p}, marks, {p->device}, &shards, &args)) != CLC_OK)
+      return rc;
+    CLC_CUDA(cudaStreamSynchronize(shards[0].p->stream));
+    if ((rc = set_device(p)) != CLC_OK) return rc;
+    rc = bench_loop(p, 1, flush_l2, flush_smem, &gather_ms[i], [&]() { return trim_launch(args[0], p->stream); });
+    if (rc != CLC_OK) return rc;
   }
-  return rc;
+  return CLC_OK;
 }
 
 int clc_bench_quantiles(clc_problem* p, const double pose7[7], int n_q, const double* q, int n, int flush_l2, float* ms_each,
                         float* frame_ms_each, int* passes) {
   if (!p || !pose7 || !q || n < 1 || !ms_each || !frame_ms_each || !passes) return fail(CLC_ERR_INVALID, "bad bench arguments");
   int rc = check_quantiles(pose7, n_q, q);
-  if (rc == CLC_OK) rc = set_device(p);
+  if (rc != CLC_OK) return rc;
   int flush_smem = 0;
-  if (rc == CLC_OK) rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem);
+  if ((rc = set_device(p)) != CLC_OK || (rc = bench_flush_prepare(p, flush_l2, 0, &flush_smem)) != CLC_OK) return rc;
   std::vector<double> values((size_t)n_q + (size_t)std::max<int64_t>(p->n_frames, 1) * n_q);
   int64_t n_valid = 0;
-  for (int i = 0; i < n && rc == CLC_OK; ++i) {
-    if (flush_l2) rc = bench_flush(p, i, flush_smem);
-    if (rc == CLC_OK) rc = quantiles_run(&p, 1, pose7, n_q, q, values.data(), &n_valid, passes, &ms_each[i]);
+  for (int i = 0; i < n; ++i) {
+    if (flush_l2 && (rc = bench_flush(p, i, flush_smem)) != CLC_OK) return rc;
+    if ((rc = quantiles_run(&p, 1, pose7, n_q, q, values.data(), &n_valid, passes, &ms_each[i])) != CLC_OK) return rc;
   }
-  double* d_block = nullptr;
-  if (rc == CLC_OK && cudaMallocAsync(&d_block, sizeof(double) * (size_t)std::max<int64_t>(p->n_frames, 1) * (n_q + 1), p->stream) !=
-                          cudaSuccess)
-    rc = fail(CLC_ERR_CUDA, "bench quantiles: allocation");
-  if (rc == CLC_OK)
-    rc = bench_loop(p, n, flush_l2, flush_smem, frame_ms_each, [&]() {
-      return frame_quantiles_launch(p, pose7, n_q, q, d_block, reinterpret_cast<int64_t*>(d_block + p->n_frames * n_q));
-    });
-  if (d_block) cudaFreeAsync(d_block, p->stream);
-  return rc;
+  Scratch<double> block;
+  CLC_CUDA(block.alloc(p, (size_t)std::max<int64_t>(p->n_frames, 1) * (n_q + 1)));
+  return bench_loop(p, n, flush_l2, flush_smem, frame_ms_each, [&]() {
+    return frame_quantiles_launch(p, pose7, n_q, q, block.get(), reinterpret_cast<int64_t*>(block.get() + p->n_frames * n_q));
+  });
 }
 
 // Profiling hook (not part of the reference-facing surface): one sweep with per-block globaltimer stamps.
@@ -4300,10 +4222,10 @@ int clc_debug_sweep_timing(clc_problem* p, const double pose7[7], int with_lm, i
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   if (grid_out) *grid_out = p->grid;
-  const size_t bytes = sizeof(unsigned long long) * 8 * (size_t)p->grid;
-  const size_t wbytes = sizeof(unsigned long long) * clc::kWarps * (size_t)p->grid;
-  CLC_CUDA(cudaMallocAsync(&p->timing, bytes + wbytes, p->stream));
-  CLC_CUDA(cudaMemsetAsync(p->timing, 0, bytes + wbytes, p->stream));
+  const size_t words = 8 * (size_t)p->grid, warp_words = clc::kWarps * (size_t)p->grid;
+  Scratch<unsigned long long> timing;
+  CLC_CUDA(timing.alloc(p, words + warp_words));
+  CLC_CUDA(cudaMemsetAsync(timing.get(), 0, sizeof(unsigned long long) * (words + warp_words), p->stream));
   if (flush_l2) {
     if (!p->flush_buf) {
       p->flush_n = ((int64_t)256 << 20) / sizeof(double);
@@ -4319,15 +4241,15 @@ int clc_debug_sweep_timing(clc_problem* p, const double pose7[7], int with_lm, i
   clc::lm_init(&p->h_lm->core, pose7, opt);
   CLC_CUDA(cudaMemcpyAsync(p->lm, p->h_lm, sizeof(clc::LmState), cudaMemcpyHostToDevice, p->stream));
   CLC_CUDA(cudaMemcpyAsync(p->pose, pose7, sizeof(double) * 7, cudaMemcpyHostToDevice, p->stream));
+  p->timing = timing.get();  // only this sweep writes its stamps
   rc = launch_sweep(p, clc::kModeLM, p->loss_kind, p->n_edges > 0, p->pose, nullptr, with_lm ? p->lm : nullptr, /*collective=*/false);
-  cudaError_t e = cudaMemcpyAsync(stamps, p->timing, bytes, cudaMemcpyDeviceToHost, p->stream);
-  if (e == cudaSuccess && warp_stamps)
-    e = cudaMemcpyAsync(warp_stamps, p->timing + 8 * (size_t)p->grid, wbytes, cudaMemcpyDeviceToHost, p->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-  cudaFreeAsync(p->timing, p->stream);
   p->timing = nullptr;
   if (rc != CLC_OK) return rc;
-  if (e != cudaSuccess) return fail(CLC_ERR_CUDA, cudaGetErrorString(e));
+  CLC_CUDA(cudaMemcpyAsync(stamps, timing.get(), sizeof(unsigned long long) * words, cudaMemcpyDeviceToHost, p->stream));
+  if (warp_stamps)
+    CLC_CUDA(cudaMemcpyAsync(warp_stamps, timing.get() + words, sizeof(unsigned long long) * warp_words, cudaMemcpyDeviceToHost,
+                             p->stream));
+  CLC_CUDA(cudaStreamSynchronize(p->stream));
   return CLC_OK;
 }
 
