@@ -12,7 +12,7 @@ SOURCES = ["clc_api.cu", "clc_pack.cpp"]
 HEADERS = ["clc_kernels.cuh", "clc_math.cuh", "clc_lm.cuh", "clc_expand.cuh", "clc_linefit.cuh", "clc_camera.cuh", "clc_upload.inl", "clc_l2_plan.h", "clc_frames.cuh",
            "clc_subset.cuh", "clc_subset_plan.h", "clc_trim.cuh", "clc_trim_plan.h", "clc_segments.cuh", "clc_segment_plan.h",
            "clc_small.cuh", "clc_small_body.inl", "clc_time_offset.cuh", "clc_select.cuh",
-           "clc_quantiles.cuh", "clc_quantile_plan.h"]
+           "clc_quantiles.cuh", "clc_quantile_plan.h", "clc_range_bias.cuh"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

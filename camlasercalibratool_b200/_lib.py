@@ -228,6 +228,12 @@ SIGNATURES = {
                                               c_double_p]),
     "clc_solve_lm_time_offset": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(LmOptions), C.POINTER(LmSummary),
                                            C.POINTER(LmIteration), C.c_int]),
+    "clc_eval_range_bias": (C.c_int, [_P, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p]),
+    "clc_information_range_bias": (C.c_int, [_P, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p,
+                                             c_double_p]),
+    "clc_solve_lm_range_bias": (C.c_int, [_P, c_double_p, c_double_p, C.POINTER(LmOptions), C.POINTER(LmSummary),
+                                          C.POINTER(LmIteration), C.c_int]),
+    "clc_problem_range_correct": (C.c_int, [_P, c_double_p, C.POINTER(_P)]),
     "clc_scan_segments": (C.c_int,[C.POINTER(C.c_float), C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_double,
                                     C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]),
     "clc_estimate_board_poses": (C.c_int, [C.POINTER(CameraDesc), C.c_int64, c_int64_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
@@ -247,6 +253,7 @@ SIGNATURES = {
     "clc_bench_segments": (C.c_int, [_P, C.c_int64, c_int64_p, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_poses": (C.c_int, [_P, C.c_int64, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_time_offset": (C.c_int, [_P, c_double_p, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_float)]),
+    "clc_bench_range_bias": (C.c_int, [_P, c_double_p, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_subset": (C.c_int, [_P, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.POINTER(C.c_float)]),
     "clc_bench_trim": (C.c_int, [_P, c_double_p, c_double_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     "clc_problem_algorithmic_bytes": (C.c_int, [_P, c_int64_p]),

@@ -374,6 +374,37 @@ def time_offset_mask(fixed) -> int:
     return mask
 
 
+RANGE_BIAS_NAMES = FIXED_NAMES + ("range_offset", "range_scale")  # bits 6, 7 of fixed_mask hold b, s in solve_range_bias only
+
+
+def range_bias_mask(fixed) -> int:
+    """Names of the coordinates solve_range_bias holds (RANGE_BIAS_NAMES: the six of fixed_mask, then "range_offset" b and
+    "range_scale" s) -> its fixed_mask, any proper subset of the eight."""
+    if isinstance(fixed, str):
+        fixed = (fixed,)
+    mask = 0
+    for name in fixed:
+        if name not in RANGE_BIAS_NAMES:
+            raise ValueError(f"unknown coordinate {name!r}: the names are {' '.join(RANGE_BIAS_NAMES)}")
+        mask |= 1 << RANGE_BIAS_NAMES.index(name)
+    if mask == (1 << 8) - 1:
+        raise ValueError("holding all eight coordinates leaves nothing to solve")
+    return mask
+
+
+def _pose_bias(pose7, bias):
+    """The float64 pose7 [7] and bias (b, s) [2] of the range-bias calls, checked before any library call."""
+    x = np.ascontiguousarray(pose7, dtype=np.float64).reshape(-1)
+    if x.shape != (7,):
+        raise ValueError("pose7 must have 7 entries")
+    b = np.ascontiguousarray(bias, dtype=np.float64).reshape(-1)
+    if b.shape != (2,):
+        raise ValueError("bias must be (range_offset, range_scale)")
+    if not (np.all(np.isfinite(x)) and np.all(np.isfinite(b))):
+        raise ValueError("pose7 and bias must be finite")
+    return x, b
+
+
 def _trajectory(knot_times, knot_poses, frame_times, n_frames):
     """The float64 arrays of clc_problem_set_trajectory (checked before any device work: the library checks them too)."""
     t = np.ascontiguousarray(knot_times, dtype=np.float64)
@@ -747,6 +778,58 @@ class Problem:
                    "clc_solve_lm_time_offset")
         return x, t.value, s, [tr[i] for i in range(min(s.num_iterations, trace_cap))] if trace_cap > 0 else []
 
+    # ---- the laser's range offset and scale ----
+    def eval_range_bias(self, pose7, bias):
+        """eval() with every point p moved to kappa p along its ray, kappa = 1 + s + b / |p| (bias = (b, s): the range offset in
+        the points' unit and the range scale; clc_eval_range_bias).  Returns (cost, H [8, 8], g [8]) over (tx ty tz rx ry rz b
+        s)."""
+        x, b = _pose_bias(pose7, bias)
+        H, g, cost = np.empty((8, 8)), np.empty(8), C.c_double()
+        _lib.check(self._L.clc_eval_range_bias(self._h, _dp(x), _dp(b), _dp(H), _dp(g), C.byref(cost)), "clc_eval_range_bias")
+        return cost.value, H, g
+
+    def information_range_bias(self, pose7, bias):
+        """information() with the range bias (clc_information_range_bias): (H [8, 8], b [8], chi, sv [8]); the right singular
+        vectors go to self.last_V [8, 8].  A small singular value whose V column lies in the span of the translation, e_b and
+        e_s: the boards were seen in too narrow a band of ranges to tell the scale from the offset."""
+        x, bb = _pose_bias(pose7, bias)
+        H, b, sv, chi = np.empty((8, 8)), np.empty(8), np.empty(8), C.c_double()
+        self.last_V = np.empty((8, 8))
+        _lib.check(self._L.clc_information_range_bias(self._h, _dp(x), _dp(bb), _dp(H), _dp(b), C.byref(chi), _dp(sv),
+                                                      _dp(self.last_V)), "clc_information_range_bias")
+        return H, b, chi.value, sv
+
+    def solve_range_bias(self, pose7, bias=(0.0, 0.0), options: LmOptions | None = None, fixed=None, trace_cap=256):
+        """solve() of the extrinsic with the laser's range offset b and scale s (clc_solve_lm_range_bias).  fixed: names of
+        RANGE_BIAS_NAMES held at their start values for this call (overrides options.fixed_mask); e.g. fixed="range_scale"
+        estimates the offset alone.  Returns (pose7, bias (b, s), summary, trace)."""
+        x, b = _pose_bias(pose7, bias)
+        x, b = x.copy(), b.copy()
+        if not 0 <= int(trace_cap) <= 256:
+            raise ValueError("trace_cap must be in [0, 256]")
+        o = LmOptions.from_buffer_copy(options) if options is not None else default_options()  # the caller's stays as it is
+        if fixed is not None:
+            o.fixed_mask = range_bias_mask(fixed)
+        s = LmSummary()
+        tr = (LmIteration * trace_cap)() if trace_cap > 0 else None
+        _lib.check(self._L.clc_solve_lm_range_bias(self._h, _dp(x), _dp(b), C.byref(o), C.byref(s), tr, int(trace_cap)),
+                   "clc_solve_lm_range_bias")
+        return x, b, s, [tr[i] for i in range(min(s.num_iterations, trace_cap))] if trace_cap > 0 else []
+
+    def range_corrected(self, bias):
+        """A new problem whose points are this one's moved to kappa p, kappa = 1 + s + b / |p| (clc_problem_range_correct), built
+        on the device from this one's points -- no upload.  Every other call (trim, quantiles, frame_report, select_frames,
+        segments, starts) then runs on the corrected points.  This problem is unchanged; close the new one when it is no longer
+        needed."""
+        b = np.ascontiguousarray(bias, dtype=np.float64).reshape(-1)
+        if b.shape != (2,) or not np.all(np.isfinite(b)):
+            raise ValueError("bias must be finite (range_offset, range_scale)")
+        if not 1.0 + b[1] > 0.0:
+            raise ValueError("1 + range_scale must be positive")
+        h = C.c_void_p()
+        _lib.check(self._L.clc_problem_range_correct(self._h, _dp(b), C.byref(h)), "clc_problem_range_correct")
+        return Problem(h)
+
     def closed_form(self):
         T, AtA, Atb, un = np.empty(16), np.empty((9, 9)), np.empty(9), C.c_int()
         _lib.check(self._L.clc_closed_form(self._h, _dp(T), C.byref(un), _dp(AtA), _dp(Atb)), "clc_closed_form")
@@ -814,6 +897,14 @@ class Problem:
         ms = (C.c_float * n)()
         _lib.check(self._L.clc_bench_time_offset(self._h, _dp(pose7), float(td), int(n), int(bool(flush_l2)), ms),
                    "clc_bench_time_offset")
+        return np.array(ms[:], dtype=np.float64)
+
+    def bench_range_bias(self, pose7, bias, n, flush_l2=True):
+        """Device time of n range-bias iterations (frame constants, range sweep, fix-up, two-level reduction;
+        clc_bench_range_bias), ms each."""
+        x, b = _pose_bias(pose7, bias)
+        ms = (C.c_float * n)()
+        _lib.check(self._L.clc_bench_range_bias(self._h, _dp(x), _dp(b), int(n), int(bool(flush_l2)), ms), "clc_bench_range_bias")
         return np.array(ms[:], dtype=np.float64)
 
     def bench_subset(self, keep, n, flush_l2=True):

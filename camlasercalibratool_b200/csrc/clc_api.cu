@@ -33,6 +33,7 @@
 #include "clc_subset.cuh"
 #include "clc_subset_plan.h"
 #include "clc_time_offset.cuh"
+#include "clc_range_bias.cuh"
 #include "clc_trim.cuh"
 
 namespace {
@@ -487,12 +488,12 @@ int launch_sweep(clc_problem* p, int mode, int loss, bool edges, const double* d
     if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
-  } else if (mode == clc::kModeSegments) {
-    // the segmented solves: no LM state in the kernel, no L2 hints, never collective
+  } else if (mode == clc::kModeSegments || mode == clc::kModeRange) {
+    // the segmented solves and the range bias: no LM state in the kernel, no L2 hints, never collective
     if (frame_rows == nullptr || frame_slots == nullptr || seg_consts == nullptr || d_lm != nullptr || loop_sweeps > 1 ||
         a.nranks > 1)
       return fail(CLC_ERR_INVALID, "internal: bad segmented sweep");
-    const SweepFn fn = sweep_fn<clc::kModeSegments>(loss, p->planar);
+    const SweepFn fn = mode == clc::kModeRange ? sweep_fn<clc::kModeRange>(loss, p->planar) : sweep_fn<clc::kModeSegments>(loss, p->planar);
     if (fn == nullptr) return fail(CLC_ERR_INVALID, "internal: unknown loss kind");
     CLC_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
     le = cudaLaunchKernelEx(&cfg, fn, v, a);
@@ -1662,12 +1663,13 @@ int solve_finish(clc_problem* p, double pose7[7], clc_lm_summary* summary, clc_l
   return CLC_OK;
 }
 
-// the first check of every LM entry point, before its other arguments and any device work (D: the solve's tangent columns, 6 or
-// 7 with the time offset)
+// the first check of every LM entry point, before its other arguments and any device work (D: the solve's tangent columns, 6,
+// 7 with the time offset, 8 with the range bias)
 int check_fixed_mask(const clc_lm_options* opt, int D = 6) {
   if (opt && (opt->fixed_mask < 0 || opt->fixed_mask >= (1 << D) - 1))
-    return fail(CLC_ERR_INVALID, D == 6 ? "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)"
-                                        : "fixed_mask must hold a proper subset of the seven coordinates (0 <= mask < 127)");
+    return fail(CLC_ERR_INVALID, D == 6   ? "fixed_mask must hold a proper subset of the six tangent coordinates (0 <= mask < 63)"
+                                 : D == 7 ? "fixed_mask must hold a proper subset of the seven coordinates (0 <= mask < 127)"
+                                          : "fixed_mask must hold a proper subset of the eight coordinates (0 <= mask < 255)");
   return CLC_OK;
 }
 
@@ -1814,8 +1816,10 @@ struct SegmentRun {
 };
 
 // the plan, the work buffers and the problem's eval pose (which the sweep does not use) on the device; rows and partials are
-// `width` doubles wide (the time-offset calls expand every frame into kTdSums)
-int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, SegmentRun* r, int width = clc::kNumSums) {
+// `width` doubles wide (the time-offset calls expand every frame into kTdSums), raw rows and slots `raw_width` and `slot_width`
+// (the range-bias sweep leaves kRangeRawDoubles)
+int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, SegmentRun* r, int width = clc::kNumSums,
+                     int raw_width = clc::kSegRawDoubles, int slot_width = clc::kSlotDoubles) {
   int rc = set_device(p);
   if (rc != CLC_OK) return rc;
   r->p = p;
@@ -1827,9 +1831,9 @@ int segments_prepare(clc_problem* p, int64_t W, const int64_t* seg_offsets, Segm
   CLC_CUDA(r->chunk_offsets.alloc(p, plan.chunk_offsets.size()));
   CLC_CUDA(r->seg_chunks.alloc(p, plan.seg_chunks.size()));
   CLC_CUDA(r->consts.alloc(p, (N + (size_t)p->n_edges) * 4));
-  CLC_CUDA(r->raw.alloc(p, N * clc::kSegRawDoubles));
+  CLC_CUDA(r->raw.alloc(p, N * raw_width));
   CLC_CUDA(r->rows.alloc(p, N * width));
-  CLC_CUDA(r->slots.alloc(p, (size_t)p->grid * clc::kWarps * 2 * clc::kSlotDoubles));
+  CLC_CUDA(r->slots.alloc(p, (size_t)p->grid * clc::kWarps * 2 * slot_width));
   CLC_CUDA(r->partials.alloc(p, (size_t)r->n_chunks * width));
   // pageable sources: each copy has read its source when it returns
   if (N > 0)
@@ -2147,6 +2151,122 @@ int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const 
   if (rc != CLC_OK) return rc;
   for (int i = 0; i < 7; ++i) pose7[i] = x8[i];
   *td = x8[7];
+  return CLC_OK;
+}
+
+// ---- the laser's range offset and scale (clc_range_bias.cuh) ---------------------------------------------------------
+// Every problem size runs it on the sweep kernel K1 (kModeRange) with the kernel family eval uses, as one segment of all frames:
+// segments_prepare's plan and buffers with seg_offsets = {0, n_frames}, raw rows and slots kRangeRawDoubles wide, rows and
+// partials kRangeSums wide.
+
+namespace {
+
+// rejects bad arguments before the device is touched (pose7 and bias2 = (b, s): the point of an evaluation, or the start of a
+// solve)
+int check_range_bias(const clc_problem* p, const double* pose7, const double* bias2) {
+  if (!p || !pose7 || !bias2) return fail(CLC_ERR_INVALID, "NULL argument");
+  if (p->n_edges > 0) return fail(CLC_ERR_INVALID, "range-bias calls take a problem without edge residuals");
+  if (p->comm_obj != nullptr || p->nranks > 1) return fail(CLC_ERR_STATE, "range-bias calls run on a problem without a communicator");
+  for (int i = 0; i < 7; ++i)
+    if (!clc::is_finite(pose7[i])) return fail(CLC_ERR_INVALID, "a pose7 entry is not finite");
+  if (!clc::is_finite(bias2[0]) || !clc::is_finite(bias2[1])) return fail(CLC_ERR_INVALID, "a bias2 entry is not finite");
+  return CLC_OK;
+}
+
+// The device buffers of one range-bias call: SegmentRun over one segment of every frame (poses: the point (pose7, b, s) of an
+// evaluation, sums: its kRangeSums sums), plus the solve's LM state.
+struct RangeRun {
+  SegmentRun s;
+  Scratch<clc::LmCoreRange> core;  // solve
+};
+
+int range_prepare(clc_problem* p, RangeRun* r) {
+  const int64_t off[2] = {0, p->n_frames};
+  return segments_prepare(p, 1, off, &r->s, clc::kRangeSums, clc::kRangeRawDoubles, clc::kRangeRawDoubles);
+}
+
+// One iteration at x9 = (pose7, b, s) on the device.  sums: [kRangeSums] or nullptr; core: the solve's LM state (lm_update runs on
+// it), with its trace and counters (running, done) as segments_iteration's.
+int range_iteration(const RangeRun& r, int loss, const double* x9, double* sums, clc::LmCoreRange* core, clc_lm_iteration* trace,
+                    int trace_cap, int* counters) {
+  clc_problem* p = r.s.p;
+  int* done = counters != nullptr ? counters + 1 : nullptr;
+  const clc::ProblemView v = make_view(p);
+  const int threads = 256;
+  if (p->n_frames > 0) {
+    const unsigned fb = (unsigned)((p->n_frames + threads - 1) / threads);
+    clc::clc_segment_consts_kernel<<<fb, threads, 0, p->stream>>>(v, r.s.frame_seg.get(), x9, 0, 0, done, r.s.consts.get());
+    CLC_LAUNCH_CHECK();
+    int rc = launch_sweep(p, clc::kModeRange, loss, false, x9, done, nullptr, /*collective=*/false, /*pdl=*/false,
+                          /*loop_sweeps=*/1, /*l2_hints=*/false, r.s.raw.get(), r.s.slots.get(), r.s.consts.get());
+    if (rc != CLC_OK) return rc;
+    const auto fixup = loss_instance(loss, [](auto L) { return clc::clc_range_fixup_kernel<L.value>; });
+    fixup<<<fb, threads, 0, p->stream>>>(v, r.s.consts.get(), x9, done, r.s.raw.get(), r.s.slots.get(), r.s.rows.get());
+    CLC_LAUNCH_CHECK();
+  }
+  return segments_reduce(r.s, sums, core, trace, trace_cap, counters, done);
+}
+
+// An evaluation at (pose7, b, s) (which: 0 eval with the problem's loss, 1 information -- no loss): its buffers in r, its one
+// iteration in *iterate.
+int range_eval_prepare(clc_problem* p, const double* pose7, const double* bias2, int which, RangeRun* r,
+                       std::function<int()>* iterate) {
+  int rc = check_range_bias(p, pose7, bias2);
+  if (rc != CLC_OK) return rc;
+  const double x9[9] = {pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6], bias2[0], bias2[1]};
+  if ((rc = range_prepare(p, r)) != CLC_OK || (rc = eval_points<8>(&r->s, 1, x9)) != CLC_OK) return rc;
+  const int loss = which == 0 ? p->loss_kind : clc::kLossNone;
+  *iterate = [r, loss]() { return range_iteration(*r, loss, r->s.poses.get(), r->s.sums.get(), nullptr, nullptr, 0, nullptr); };
+  return CLC_OK;
+}
+
+}  // namespace
+
+int clc_eval_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], double H64[64], double g8[8], double* cost) {
+  RangeRun r;
+  std::function<int()> iterate;
+  const int rc = range_eval_prepare(p, pose7, bias2, 0, &r, &iterate);
+  if (rc != CLC_OK) return rc;
+  return eval_items<8>(r.s, 1, iterate, [&](const double* sums, int64_t) { eval_post<8>(sums, H64, g8, cost); });
+}
+
+int clc_information_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], double H64[64], double b8[8], double* chi,
+                               double singular_values8[8], double V64[64]) {
+  RangeRun r;
+  std::function<int()> iterate;
+  const int rc = range_eval_prepare(p, pose7, bias2, 1, &r, &iterate);
+  if (rc != CLC_OK) return rc;
+  return eval_items<8>(r.s, 1, iterate,
+                       [&](const double* sums, int64_t) { information_post<8>(sums, H64, b8, chi, singular_values8, V64); });
+}
+
+int clc_solve_lm_range_bias(clc_problem* p, double pose7[7], double bias2[2], const clc_lm_options* opt_in, clc_lm_summary* summary,
+                            clc_lm_iteration* trace, int trace_cap) {
+  if (check_fixed_mask(opt_in, 8) != CLC_OK) return CLC_ERR_INVALID;
+  if (trace_cap < 0 || trace_cap > clc::kTraceMax || (trace_cap > 0 && !trace))
+    return fail(CLC_ERR_INVALID, "trace_cap outside [0, 256], or without a trace array");
+  int rc = check_range_bias(p, pose7, bias2);
+  if (rc != CLC_OK) return rc;
+  clc_lm_options opt;
+  if ((rc = lm_options(opt_in, &opt, 8)) != CLC_OK) return rc;
+  RangeRun r;
+  if ((rc = range_prepare(p, &r)) != CLC_OK) return rc;
+  CLC_CUDA(r.core.alloc(p, 1));
+  CLC_CUDA(r.s.counters.alloc(p, 2));
+  if (trace_cap > 0) CLC_CUDA(r.s.trace.alloc(p, trace_cap));
+  const int counters0[2] = {1, 0};
+  CLC_CUDA(cudaMemcpyAsync(r.s.counters.get(), counters0, sizeof(counters0), cudaMemcpyHostToDevice, p->stream));
+  const int loss = p->loss_kind;
+  double x9[9] = {pose7[0], pose7[1], pose7[2], pose7[3], pose7[4], pose7[5], pose7[6], bias2[0], bias2[1]};
+  rc = lm_solve_items<8>(p, 1, opt, x9, r.core.get(), r.s.trace.get(), trace_cap, r.s.counters.get(),
+                         [&](const double* cand, int64_t) {  // cand: (pose7, b, s) of the next sweep
+                           return range_iteration(r, loss, cand, nullptr, r.core.get(), r.s.trace.get(), trace_cap, r.s.counters.get());
+                         },
+                         summary, trace);
+  if (rc != CLC_OK) return rc;
+  for (int i = 0; i < 7; ++i) pose7[i] = x9[i];
+  bias2[0] = x9[7];
+  bias2[1] = x9[8];
   return CLC_OK;
 }
 
@@ -3447,6 +3567,45 @@ int clc_problem_subset(const clc_problem* src, const uint8_t* keep, clc_problem*
   return CLC_OK;
 }
 
+// ---- the range-corrected copy of a problem (clc_range_bias.cuh) --------------------------------------------------
+
+namespace {
+
+// The correction of a copy's points in place, on its stream: kappa p for every point (clc_range_correct_kernel).
+int range_correct_launch(clc_problem* p, double b, double s) {
+  if (p->n_points == 0) return CLC_OK;
+  const int threads = 256;
+  const int64_t pairs = (p->n_points + 1) / 2;
+  const int64_t blocks = std::min<int64_t>((pairs + threads - 1) / threads, (int64_t)std::max(p->num_sms, 1) * 8);
+  clc::clc_range_correct_kernel<<<(unsigned)blocks, threads, 0, p->stream>>>(p->x, p->y, p->z, p->n_points, b, s, p->x, p->y, p->z);
+  CLC_LAUNCH_CHECK();
+  return CLC_OK;
+}
+
+}  // namespace
+
+int clc_problem_range_correct(const clc_problem* src, const double bias2[2], clc_problem** out) {
+  if (!src || !bias2 || !out) return fail(CLC_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  if (!clc::is_finite(bias2[0]) || !clc::is_finite(bias2[1])) return fail(CLC_ERR_INVALID, "a bias2 entry is not finite");
+  if (!(1.0 + bias2[1] > 0.0)) return fail(CLC_ERR_INVALID, "1 + s must be positive");
+  if (src->n_edges > 0) return fail(CLC_ERR_INVALID, "range-bias calls take a problem without edge residuals");
+  // every frame kept: the subset gather copies the points and the per-frame arrays, the correction then runs in place on the copy
+  const std::vector<uint8_t> keep((size_t)src->n_frames, 1);
+  std::vector<SubsetShard> shards;
+  const std::vector<clc_problem*> from = {const_cast<clc_problem*>(src)};
+  int rc = subset_prepare(from, keep.data(), {src->device}, &shards);
+  if (rc == CLC_OK)
+    rc = gather_shards(from, {src->device}, shards, [&](size_t d) {
+      const int lrc = subset_launch(shards[d], shards[d].p->stream);
+      return lrc != CLC_OK ? lrc : range_correct_launch(shards[d].p, bias2[0], bias2[1]);
+    });
+  std::vector<clc_problem*> ps;
+  if ((rc = finish_shards(shards, rc, &ps)) != CLC_OK) return rc;
+  *out = ps[0];
+  return CLC_OK;
+}
+
 int clc_group_subset(const clc_group* src, const uint8_t* keep, clc_group** out) {
   if (!src || !keep || !out) return fail(CLC_ERR_INVALID, "NULL argument");
   *out = nullptr;
@@ -4114,6 +4273,18 @@ int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int 
   TimeRun r;
   std::function<int()> iterate;
   int rc = time_eval_prepare(p, pose7, td, 0, &r, &iterate);
+  if (rc != CLC_OK) return rc;
+  int flush_smem = 0;
+  rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);
+  if (rc != CLC_OK) return rc;
+  return bench_loop(p, n, flush_l2, flush_smem, ms_each, iterate);
+}
+
+int clc_bench_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], int n, int flush_l2, float* ms_each) {
+  if (n < 1 || !ms_each) return fail(CLC_ERR_INVALID, "bad bench arguments");
+  RangeRun r;
+  std::function<int()> iterate;
+  int rc = range_eval_prepare(p, pose7, bias2, 0, &r, &iterate);
   if (rc != CLC_OK) return rc;
   int flush_smem = 0;
   rc = bench_flush_prepare(p, flush_l2, clc::dyn_smem_bytes(p->planar), &flush_smem);

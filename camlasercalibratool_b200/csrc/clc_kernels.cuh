@@ -9,6 +9,8 @@
 
 #include <cuda_runtime.h>
 
+#include <type_traits>
+
 #include "clc_camera.cuh"
 #include "clc_expand.cuh"
 #include "clc_frames.cuh"
@@ -88,7 +90,13 @@ constexpr int kSegRawDoubles = 12;
 // place of the tile (12 doubles per pose: 10 moments, cost, exponent).
 constexpr int kPoseTile = 32;
 static_assert(kPoseTile * kSegRawDoubles <= kTileDoublesPerWarp, "the open pieces of a pose tile live in the warp's tile");
-enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3, kModePoses = 4 };
+// kModeRange: the extrinsic with the laser's range offset and scale (clc_range_bias.cuh) -- as kModeSegments, with the frame
+// constants of SweepArgs::seg_consts, but every point is first moved to kappa p (kappa = 1 + s + b / r, (b, s) = pose7[7], [8]:
+// the LM candidate) and every piece leaves kRangeRawDoubles: the 25 RangeMoments, the cost and its exponent.  A split frame's
+// pieces go to per-warp head / tail slots of the same width.
+constexpr int kRangeMoments = 25;
+constexpr int kRangeRawDoubles = kRangeMoments + 2;
+enum SweepMode { kModeLM = 0, kModeClosedForm = 1, kModeFrames = 2, kModeSegments = 3, kModePoses = 4, kModeRange = 5 };
 
 // Device-resident problem (read-only for the sweeps).
 struct ProblemView {
@@ -139,7 +147,8 @@ struct SweepArgs {
   // kModeFrames only
   double* frame_rows;   // [n_frames * kRowDoubles] the report rows of the frames that lie in one warp range
   double* frame_slots;  // [total warps * 2 * kSlotDoubles] head / tail pieces of split frames (clc_frames.cuh)
-  // kModeSegments only (frame_rows then holds [n_frames * kSegRawDoubles] raw rows; frame_slots as above)
+  // kModeSegments only (frame_rows then holds [n_frames * kSegRawDoubles] raw rows; frame_slots as above); kModeRange: rows and
+  // slots kRangeRawDoubles wide, and pose7 points at (pose7, b, s)
   const double* seg_consts;  // [(n_frames + n_edges) * 4] m, c of every frame, then of every edge residual, at its segment's pose
   // kModePoses only: pose k's constants at seg_consts + k * pose_consts_stride, its raw rows at frame_rows + k * pose_rows_stride,
   // its slots at frame_slots + k * pose_slots_stride; this launch walks the poses pose_active[pose_tile0 ..
@@ -325,6 +334,66 @@ __device__ __forceinline__ void accumulate(Moments& a, double w, double x, doubl
   }
 }
 
+// The robust weights w0, w1 of two residuals e0, e1 (v0/v1: validity of the two points; an invalid point gets w = 0) and their
+// cost terms added to prod (Cauchy: multiplied into it), with process2's arithmetic operation for operation.  LOSS: LossKind
+// (clc_expand.cuh); COST: the no-loss kind also sums e^2.  ha: the loss parameter (Huber only), a2 = ha^2.  (process2 keeps its
+// own inline copy: calling this from it changes the SASS of its no-loss and soft-L1 instantiations.)
+template <int LOSS, bool COST>
+__device__ __forceinline__ void weigh2(double& prod, double e0, double e1, bool v0, bool v1, double inv_a2, double ha, double a2,
+                                       double& w0, double& w1) {
+  if (LOSS == kLossHuber) {
+    // w = a / max(|e|, a): one reciprocal of the product of the two denominators serves both weights (a NaN e stays NaN)
+    const double ae0 = fabs(e0), ae1 = fabs(e1);
+    double d0 = ae0 < ha ? ha : ae0, d1 = ae1 < ha ? ha : ae1;
+    d0 = v0 ? d0 : ha;
+    d1 = v1 ? d1 : ha;
+    const double ar = ha * rcp_pos(d0 * d1);
+    w0 = ar * d1;
+    w1 = ar * d0;
+    w0 = v0 ? w0 : 0.0;
+    w1 = v1 ? w1 : 0.0;
+    // rho~ = e^2 inside a, 2 a |e| - a^2 outside: summed directly, like e^2 without a loss
+    const double r0 = ae0 <= ha ? e0 * e0 : fma(2.0 * ha, ae0, -a2);
+    const double r1 = ae1 <= ha ? e1 * e1 : fma(2.0 * ha, ae1, -a2);
+    prod += v0 ? r0 : 0.0;
+    prod += v1 ? r1 : 0.0;
+  } else if (LOSS == kLossSoftL1) {
+    // w = 1/sqrt(u), u = 1 + e^2/a^2; rho~ = 2 e^2 / (1 + sqrt(u)) with sqrt(u) = u w -- one reciprocal for both points
+    double u0 = fma(e0 * inv_a2, e0, 1.0);
+    double u1 = fma(e1 * inv_a2, e1, 1.0);
+    u0 = v0 ? u0 : 1.0;
+    u1 = v1 ? u1 : 1.0;
+    const double y0 = rsqrt(u0), y1 = rsqrt(u1);
+    const double t0 = fma(u0, y0, 1.0), t1 = fma(u1, y1, 1.0);
+    const double r = rcp_pos(t0 * t1);
+    const double r0 = (2.0 * e0) * e0 * (r * t1), r1 = (2.0 * e1) * e1 * (r * t0);
+    prod += v0 ? r0 : 0.0;
+    prod += v1 ? r1 : 0.0;
+    w0 = v0 ? y0 : 0.0;
+    w1 = v1 ? y1 : 0.0;
+  } else if (LOSS == kLossCauchy) {
+    double u0 = fma(e0 * inv_a2, e0, 1.0);
+    double u1 = fma(e1 * inv_a2, e1, 1.0);
+    u0 = v0 ? u0 : 1.0;
+    u1 = v1 ? u1 : 1.0;
+    // batch inversion: one reciprocal of u0*u1 serves both weights and the cost product
+    const double p = u0 * u1;
+    const double r = rcp_pos(p);
+    w0 = r * u1;
+    w1 = r * u0;
+    w0 = v0 ? w0 : 0.0;
+    w1 = v1 ? w1 : 0.0;
+    prod *= p;
+  } else {
+    if (COST) {
+      prod = fma(v0 ? e0 : 0.0, e0, prod);
+      prod = fma(v1 ? e1 : 0.0, e1, prod);
+    }
+    w0 = v0 ? 1.0 : 0.0;
+    w1 = v1 ? 1.0 : 0.0;
+  }
+}
+
 // Two points (one LDG.128 per coordinate array).  v0/v1: validity of the two points.  LOSS: LossKind (clc_expand.cuh); COST:
 // the no-loss kind also sums e^2 (the other kinds always sum their cost term).  a: the loss parameter (Huber only), a2 = a^2.
 template <int LOSS, bool COST, bool PLANAR>
@@ -387,6 +456,64 @@ __device__ __forceinline__ void process2(Moments& a, const double2 X, const doub
     accumulate<PLANAR>(a, v0 ? 1.0 : 0.0, X.x, Y.x, Z.x);
     accumulate<PLANAR>(a, v1 ? 1.0 : 0.0, X.y, Y.y, Z.y);
   }
+}
+
+// kModeRange: the moments of a piece in the augmented vector a = (p, p/r, 1), r = |p| (clc_range_bias.cuh): Moments' 10
+// (1, p, p p^T), then p/r, p p^T / r and p p^T / r^2 -- 25 in all, 14 of them non-zero on a planar problem.
+struct RangeMoments : Moments {
+  double Qx, Qy, Qz;                          // sum w p / r
+  double Pxx, Pxy, Pxz, Pyy, Pyz, Pzz;        // sum w p p^T / r
+  double P2xx, P2xy, P2xz, P2yy, P2yz, P2zz;  // sum w p p^T / r^2
+};
+
+template <int LOSS>
+__device__ __forceinline__ void moments_clear(RangeMoments& a) {
+  moments_clear<LOSS>(static_cast<Moments&>(a));
+  a.Qx = a.Qy = a.Qz = 0.0;
+  a.Pxx = a.Pxy = a.Pxz = a.Pyy = a.Pyz = a.Pzz = 0.0;
+  a.P2xx = a.P2xy = a.P2xz = a.P2yy = a.P2yz = a.P2zz = 0.0;
+}
+
+// One point's share of the range moments: w, w / r, w / r^2 on the three blocks (inv_r = 1 / r, 0 at r == 0)
+template <bool PLANAR>
+__device__ __forceinline__ void accumulate_range(RangeMoments& a, double w, double inv_r, double x, double y, double z) {
+  accumulate<PLANAR>(a, w, x, y, z);
+  const double wr = w * inv_r, wrr = wr * inv_r;
+  const double rx = wr * x, ry = wr * y, qx = wrr * x, qy = wrr * y;
+  a.Qx += rx; a.Qy += ry;
+  a.Pxx = fma(rx, x, a.Pxx); a.Pxy = fma(rx, y, a.Pxy); a.Pyy = fma(ry, y, a.Pyy);
+  a.P2xx = fma(qx, x, a.P2xx); a.P2xy = fma(qx, y, a.P2xy); a.P2yy = fma(qy, y, a.P2yy);
+  if (!PLANAR) {
+    const double rz = wr * z, qz = wrr * z;
+    a.Qz += rz;
+    a.Pxz = fma(rx, z, a.Pxz); a.Pyz = fma(ry, z, a.Pyz); a.Pzz = fma(rz, z, a.Pzz);
+    a.P2xz = fma(qx, z, a.P2xz); a.P2yz = fma(qy, z, a.P2yz); a.P2zz = fma(qz, z, a.P2zz);
+  }
+}
+
+// 1 / r of a point with r^2 = x^2 + y^2 + z^2: one FP64 reciprocal square root; 0 at r == 0 (the p / r terms of the origin are
+// 0), NaN for a NaN coordinate
+__device__ __forceinline__ double range_inv_r(double x, double y, double z) {
+  const double r2 = fma(x, x, fma(y, y, z * z));
+  return r2 == 0.0 ? 0.0 : rsqrt(r2);
+}
+
+// kModeRange's process2: the same two points at the corrected positions kappa p, kappa = sigma + b / r (sigma = 1 + s), so
+// e = kappa (m.p) + c.  Every residual of the loss is weighed as process2 weighs it (weigh2, COST = true).
+template <int LOSS, bool PLANAR>
+__device__ __forceinline__ void process2_range(RangeMoments& a, const double2 X, const double2 Y, const double2 Z, bool v0, bool v1,
+                                               double m0, double m1, double m2, double c, double sigma, double b, double inv_a2,
+                                               double ha, double a2) {
+  const double ir0 = range_inv_r(X.x, Y.x, PLANAR ? 0.0 : Z.x);
+  const double ir1 = range_inv_r(X.y, Y.y, PLANAR ? 0.0 : Z.y);
+  const double y0 = fma(m0, X.x, fma(m1, Y.x, PLANAR ? 0.0 : m2 * Z.x));
+  const double y1 = fma(m0, X.y, fma(m1, Y.y, PLANAR ? 0.0 : m2 * Z.y));
+  const double e0 = fma(fma(b, ir0, sigma), y0, c);
+  const double e1 = fma(fma(b, ir1, sigma), y1, c);
+  double w0, w1;
+  weigh2<LOSS, true>(a.prod, e0, e1, v0, v1, inv_a2, ha, a2, w0, w1);
+  accumulate_range<PLANAR>(a, w0, ir0, X.x, Y.x, Z.x);
+  accumulate_range<PLANAR>(a, w1, ir1, X.y, Y.y, Z.y);
 }
 
 __device__ __forceinline__ void renormalise(Moments& a) {
@@ -785,7 +912,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     // ahead so that a frame change does not stall the stream on a global-memory round trip
     // kModeSegments: every frame's m, c were computed at its segment's pose before the sweep; they take the place of its plane
     const double* fsrc = pv.plane;
-    if constexpr (MODE == kModeSegments) fsrc = args.seg_consts;
+    if constexpr (MODE == kModeSegments || MODE == kModeRange) fsrc = args.seg_consts;
     double nx_plane[4] = {0.0, 0.0, 0.0, 0.0};
     int64_t nx_end = 0;
     auto prefetch_next = [&]() {
@@ -796,7 +923,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       }
     };
     auto set_frame_consts = [&](const double* plane) {
-      if constexpr (MODE == kModeSegments) {
+      if constexpr (MODE == kModeSegments || MODE == kModeRange) {
         m0 = plane[0]; m1 = plane[1]; m2 = plane[2]; c = plane[3];
       } else {
         double m[3];
@@ -811,10 +938,16 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
       set_frame_consts(plane);
       prefetch_next();
     }
-    Moments a;
+    std::conditional_t<MODE == kModeRange, RangeMoments, Moments> a;
     moments_clear<LOSS>(a);
     // Huber's a (sqrt(a^2) is exact, clc_expand.cuh), once per sweep
     const double huber_a = LOSS == kLossHuber ? sqrt(pv.a2) : 0.0;
+    // kModeRange: the range offset b and 1 + s of the point being evaluated
+    double range_b = 0.0, range_sigma = 1.0;
+    if constexpr (MODE == kModeRange) {
+      range_b = args.pose7[7];
+      range_sigma = 1.0 + args.pose7[8];
+    }
     bool open = false;  // the current piece has accumulated points
     FrameSums fx;       // kModeFrames only
     frame_sums_clear(fx);
@@ -822,6 +955,34 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
 
     // sums the lanes' moments of the finished piece and parks them in the tile
     auto park_piece = [&]() {
+      if constexpr (MODE == kModeRange) {
+        // as kModeSegments: every piece leaves raw, 25 moments, the cost and its exponent
+        double v[32] = {a.S0, a.Sx, a.Sy, a.Sz, a.Sxx, a.Sxy, a.Sxz, a.Syy, a.Syz, a.Szz, a.Qx, a.Qy, a.Qz,
+                        a.Pxx, a.Pxy, a.Pxz, a.Pyy, a.Pyz, a.Pzz, a.P2xx, a.P2xy, a.P2xz, a.P2yy, a.P2yz, a.P2zz,
+                        0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        double pr = a.prod;
+        int es = a.esum;
+        if (LOSS == kLossCauchy) {
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            pr *= __shfl_xor_sync(0xffffffffu, pr, o);  // 32 mantissas in [1,2): product < 2^32
+            es += __shfl_xor_sync(0xffffffffu, es, o);
+          }
+        } else {
+          v[kRangeMoments] = pr;
+        }
+        warp_transpose_sum_regs<32>(v, lane);
+        const int kind = frame_piece_kind(pv.offsets[f], f_end, p0, p1);
+        double* dst = kind == kPieceWhole
+                          ? args.frame_rows + f * kRangeRawDoubles
+                          : args.frame_slots + (gwarp * 2 + (kind == kPieceHead ? kSlotHead : kSlotTail)) * kRangeRawDoubles;
+        if (lane < kRangeMoments || (LOSS != kLossCauchy && lane == kRangeMoments)) dst[lane] = v[0];
+        if (LOSS == kLossCauchy && lane == kRangeMoments) dst[kRangeMoments] = pr;
+        if (lane == kRangeMoments + 1) dst[kRangeMoments + 1] = (double)es;
+        moments_clear<LOSS>(a);
+        open = false;
+        return;
+      }
       double v[16] = {a.S0, a.Sx, a.Sy, a.Sz, a.Sxx, a.Sxy, a.Sxz, a.Syy, a.Syz, a.Szz, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
       double pr = a.prod;
       int es = a.esum;
@@ -939,6 +1100,11 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
           // the whole stage belongs to one frame: no masks
 #pragma unroll
           for (int g = 0; g < G; ++g) {
+            if constexpr (MODE == kModeRange) {
+              process2_range<LOSS, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, range_sigma, range_b, pv.inv_a2, huber_a,
+                                           pv.a2);
+              continue;
+            }
             process2<LOSS, MODE == kModeLM || MODE == kModeSegments, PLANAR>(a, X[g], Y[g], Z[g], true, true, m0, m1, m2, c, pv.inv_a2,
                                                                             huber_a, pv.a2);
             if (MODE == kModeFrames) frame_sums2<PLANAR>(fx, X[g], Y[g], Z[g], true, true, m0, m1, m2, c);
@@ -956,6 +1122,14 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
               const double2 Ym = make_double2(v0 ? Y[g].x : 0.0, v1 ? Y[g].y : 0.0);
               const double2 Zm = make_double2(v0 ? Z[g].x : 0.0, v1 ? Z[g].y : 0.0);
               process2<LOSS, true, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, pv.inv_a2, huber_a, pv.a2);
+              continue;
+            }
+            if constexpr (MODE == kModeRange) {  // masked as kModeSegments masks (a NaN of another frame stays out)
+              const bool v0 = i0 >= q && i0 < hi, v1 = i0 + 1 >= q && i0 + 1 < hi;
+              const double2 Xm = make_double2(v0 ? X[g].x : 0.0, v1 ? X[g].y : 0.0);
+              const double2 Ym = make_double2(v0 ? Y[g].x : 0.0, v1 ? Y[g].y : 0.0);
+              const double2 Zm = make_double2(v0 ? Z[g].x : 0.0, v1 ? Z[g].y : 0.0);
+              process2_range<LOSS, PLANAR>(a, Xm, Ym, Zm, v0, v1, m0, m1, m2, c, range_sigma, range_b, pv.inv_a2, huber_a, pv.a2);
               continue;
             }
             process2<LOSS, MODE == kModeLM, PLANAR>(a, X[g], Y[g], Z[g], i0 >= q && i0 < hi, i0 + 1 >= q && i0 + 1 < hi, m0, m1, m2,
@@ -983,7 +1157,7 @@ clc_sweep_kernel(ProblemView pv, SweepArgs args) {
     flush_frames();
     return;
   }
-  if constexpr (MODE == kModeSegments) return;  // every piece has left raw (park_piece): no tile, no block reduction
+  if constexpr (MODE == kModeSegments || MODE == kModeRange) return;  // every piece has left raw (park_piece): no tile, no block reduction
   CLC_STAMP(1);
   if (args.timing != nullptr && lane == 0) args.timing[(int64_t)gridDim.x * 8 + gwarp] = globaltimer_ns();
   flush_tile();

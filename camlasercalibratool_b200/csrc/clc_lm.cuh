@@ -19,8 +19,9 @@ namespace clc {
 
 constexpr int kTraceMax = 256;
 
-// The state machine runs over D tangent columns: D = 6, the pose (its local parameterization), or D = 7, the pose and the
-// camera-laser time offset td as a plain 1-vector (clc_time_offset.cuh).  Its sums are [upper-tri H | g | cost].
+// The state machine runs over D tangent columns: D = 6, the pose (its local parameterization); D = 7, the pose and the
+// camera-laser time offset td as a plain 1-vector (clc_time_offset.cuh); D = 8, the pose and the laser's range offset b and
+// scale s (clc_range_bias.cuh).  Tangent coordinate k >= 6 is the plain parameter x[k + 1].  Its sums are [upper-tri H | g | cost].
 template <int D>
 constexpr int kLmSums = D * (D + 1) / 2 + D + 1;
 constexpr int kNumSums = kLmSums<6>;  // 21 upper-tri H + 6 g + 1 cost
@@ -39,7 +40,7 @@ struct LmCoreN {
   int num_unsuccessful;
   int sweeps;
   int pad0;
-  double x[D + 1];     // pose7 (D = 7: then td)
+  double x[D + 1];     // pose7, then the D - 6 plain parameters (td; or b, s)
   double cand[D + 1];  // the point the next sweep evaluates
   double x_cost, x_norm;
   double H[D * (D + 1) / 2], g[D];  // at x: loss-corrected, unscaled
@@ -49,7 +50,8 @@ struct LmCoreN {
   clc_lm_options opt;
 };
 using LmCore = LmCoreN<6>;
-static_assert(sizeof(LmCore) % 8 == 0 && sizeof(LmCoreN<7>) % 8 == 0, "LmCoreN is copied as 8-byte words");
+static_assert(sizeof(LmCore) % 8 == 0 && sizeof(LmCoreN<7>) % 8 == 0 && sizeof(LmCoreN<8>) % 8 == 0,
+              "LmCoreN is copied as 8-byte words");
 template <int D>
 constexpr int kLmWords = (int)(sizeof(LmCoreN<D>) / 8);
 constexpr int kLmCoreWords = kLmWords<6>;
@@ -77,7 +79,7 @@ CLC_HD double vec_norm(const double* a) {
   return sqrt(s);
 }
 
-// Ceres EvaluateGradientAndJacobian: |x - Plus(x, -g)|_inf, over the pose and (D = 7) td
+// Ceres EvaluateGradientAndJacobian: |x - Plus(x, -g)|_inf, over the pose and the plain parameters (|g_k|, k >= 6)
 template <int D>
 CLC_HD double gradient_max_norm(const double* x, const double* g) {
   double ng[6], xp[7], m = 0.0;
@@ -87,8 +89,8 @@ CLC_HD double gradient_max_norm(const double* x, const double* g) {
     const double d = fabs(x[i] - xp[i]);
     if (d > m) m = d;
   }
-  if constexpr (D == 7) {
-    const double a = fabs(g[6]);
+  for (int k = 6; k < D; ++k) {
+    const double a = fabs(g[k]);
     if (a > m) m = a;
   }
   return m;
@@ -99,7 +101,7 @@ CLC_HD double gradient_max_norm(const double* x, const double* g) {
 // then sees the free coordinates only -- gradient_max_norm (g embedded with zeros), the Jacobi-scaled system and its LM
 // diagonal, whose positive pivot makes the Cholesky step of a held coordinate exactly 0 and that of the free ones the step of
 // the reduced system (every product with a held entry is 0), and the model cost change.  Done in place on the state (shared
-// memory on the device), off the register-resident step code.  With D = 7, bit 6 holds td.
+// memory on the device), off the register-resident step code.  Bit k >= 6 holds plain parameter k (td; b, s).
 template <int D>
 CLC_HD void lm_hold(LmCoreN<D>* s, int fixed) {
 #pragma unroll 1
@@ -112,14 +114,14 @@ CLC_HD void lm_hold(LmCoreN<D>* s, int fixed) {
   }
 }
 
-// a held translation of the candidate (or td) keeps the bits of x (x + 0 would turn a -0.0 into +0.0)
+// a held translation of the candidate (or plain parameter) keeps the bits of x (x + 0 would turn a -0.0 into +0.0)
 template <int D>
 CLC_HD void lm_hold_cand(LmCoreN<D>* s, int fixed) {
 #pragma unroll 1
   for (int k = 0; k < 3; ++k)
     if (fixed >> k & 1) s->cand[k] = s->x[k];
-  if constexpr (D == 7)
-    if (fixed >> 6 & 1) s->cand[7] = s->x[7];
+  for (int k = 6; k < D; ++k)
+    if (fixed >> k & 1) s->cand[k + 1] = s->x[k + 1];
 }
 
 template <int D>
@@ -141,7 +143,7 @@ CLC_HD void lm_record(LmCoreN<D>* s, TraceRows trace, const clc_lm_iteration& it
   s->n_trace++;
 }
 
-// x0: pose7 (D = 7: then td)
+// x0: pose7, then the plain parameters
 template <int D>
 CLC_HD void lm_init(LmCoreN<D>* s, const double* x0, const clc_lm_options& opt) {
   s->done = 0; s->phase = 0; s->iteration = 0; s->num_invalid = 0; s->reuse_diagonal = 0; s->n_trace = 0;
@@ -158,8 +160,8 @@ CLC_HD void lm_init(LmCoreN<D>* s, const double* x0, const clc_lm_options& opt) 
 
 // Consumes the kLmSums<D> sums of the sweep that has just evaluated s->cand and advances the minimiser until it either
 // terminates (s->done != 0) or has a new candidate in s->cand for the next sweep.  Trace: a clc_lm_iteration* of kTraceMax
-// rows, or TraceRows.  With D = 7 the parameter tolerance measures the 8-vector (pose7, td), gradient_max_norm also takes |g_td|
-// and the candidate's td is x_td + its step.
+// rows, or TraceRows.  With D > 6 the parameter tolerance measures the (D + 1)-vector (pose7, plain parameters),
+// gradient_max_norm also takes their |g| and a candidate's plain parameter is x's plus its step.
 template <int D, class Trace>
 CLC_HD void lm_update(LmCoreN<D>* s, Trace trace, const double* sums) {
   constexpr int kH = D * (D + 1) / 2, kSums = kLmSums<D>;
@@ -313,7 +315,7 @@ CLC_HD void lm_update(LmCoreN<D>* s, Trace trace, const double* sums) {
     for (int k = 0; k < D; ++k) delta[k] = step[k] * s->scale[k];
     CLC_LM_STAMP(5);  // model cost change done
     pose_plus(s->x, delta, s->cand);
-    if constexpr (D == 7) s->cand[7] = s->x[7] + delta[6];
+    for (int k = 6; k < D; ++k) s->cand[k + 1] = s->x[k + 1] + delta[k];
     if (o.fixed_mask) lm_hold_cand(s, o.fixed_mask);
     s->model_cost_change = mcc;
     s->phase = 1;

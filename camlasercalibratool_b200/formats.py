@@ -284,7 +284,7 @@ def board_trajectory(tagpose):
     return np.array(times), np.array(poses).reshape(-1, 7)
 
 
-def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=None, time_offset=False):
+def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=None, time_offset=False, range_bias=False):
     """reference main/calibr_offline.cpp:52-197 without the rosbag: returns (Tlc, report) or (None, reason).  fixed: names of
     tangent coordinates of T_cl (api.FIXED_NAMES) held at the closed form's value in the LM solve, e.g. the unobservable
     directions a previous report named.
@@ -292,7 +292,13 @@ def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=Non
     on the same problem, from the LM result and td = 0, with every tag pose as the board trajectory and the matched scans' own
     timestamps.  Tlc is then the joint solve's; the report adds time_offset (seconds added to a laser stamp to put it on the
     camera clock), time_offset_singular_values (information_time_offset's, at the result), time_offset_summary and
-    Tlc_without_time_offset."""
+    Tlc_without_time_offset.
+    range_bias: after that solve, estimate the laser's range offset b and range scale s together with the extrinsic
+    (Problem.solve_range_bias) on all matched points (use_linefitting_data=False), from the LM result and b = s = 0.  Tlc is then
+    the joint solve's; the report adds range_offset (in the points' unit), range_scale, range_bias_singular_values
+    (information_range_bias's, at the result), range_bias_summary and Tlc_without_range_bias.  Not together with time_offset."""
+    if time_offset and range_bias:
+        raise ValueError("time_offset and range_bias are estimated one at a time")
     if len(tagpose) < 10:  # :55-59
         return None, "apriltag pose less than 10."
     obs, scan_times = observations_from_segments(select_keyframes(tagpose), scans, return_times=True)
@@ -313,6 +319,15 @@ def calibrate_offline(tagpose, scans, result_yaml=None, verbose=False, fixed=Non
         Tcl = pose7_to_T(x)
         report["time_offset"] = td
         report["time_offset_summary"] = summary
+    if range_bias:
+        report["Tlc_without_range_bias"] = np.linalg.inv(Tcl)
+        with Problem.from_observations(obs, use_linefitting_data=False) as p:
+            x, bias, summary, _ = p.solve_range_bias(T_to_pose7(Tcl), (0.0, 0.0), options, trace_cap=0)
+            report["range_bias_singular_values"] = p.information_range_bias(x, bias)[3]
+        Tcl = pose7_to_T(x)
+        report["range_offset"] = float(bias[0])
+        report["range_scale"] = float(bias[1])
+        report["range_bias_summary"] = summary
     Tlc = np.linalg.inv(Tcl)
     if result_yaml is not None:
         write_result_yaml(result_yaml, Tlc)

@@ -123,7 +123,8 @@ typedef struct {
    * from a tape measure or a drawing.  A mask with bits above 5, or with all six bits set (63), fails with CLC_ERR_INVALID
    * before any device work in clc_solve_lm, clc_group_solve_lm, clc_solve_lm_segments and clc_solve_lm_starts.  (This field
    * was `reserved` and ignored before: callers that left garbage in it now get CLC_ERR_INVALID.)  clc_solve_lm_time_offset
-   * alone also takes bit 6 (the time offset td; masks 0..126).  clc_lm_default_options sets 0. */
+   * alone also takes bit 6 (the time offset td; masks 0..126), clc_solve_lm_range_bias bits 6 and 7 (the range offset b and
+   * scale s; masks 0..254).  clc_lm_default_options sets 0. */
   int fixed_mask;
 } clc_lm_options;
 
@@ -355,6 +356,41 @@ int clc_information_time_offset(clc_problem* p, const double pose7[7], double td
 int clc_solve_lm_time_offset(clc_problem* p, double pose7[7], double* td, const clc_lm_options* opt, clc_lm_summary* summary,
                              clc_lm_iteration* trace, int trace_cap);
 
+/* ---- the laser's range offset b and range scale s, estimated with the extrinsic ----
+ * A point p the laser reported at range r = |p| along the ray u = p / r is taken to lie at range (1 + s) r + b on the same ray,
+ * whose origin is the laser's origin:
+ *   p' = (1 + s) p + b u = kappa p,   kappa = (1 + s) + b / r;
+ * at r == 0 the p / r terms are 0 and p' = (1 + s) p = 0.  A NaN coordinate propagates as everywhere else.  The residual is the
+ * reference's at p': e = kappa (m.p) + c (m = R_cl^T n, c = n.t_cl + d), scaled by 1/sqrt(#points), with the problem's loss.  The
+ * tangent space is (tx ty tz rx ry rz b s): the pose columns at p', de/db = (m.p) / r, de/ds = m.p.  H64 / V64 are row-major 8x8
+ * over it, g8 / b8 likewise; bias2 = (b, s), b in the points' unit.  Every problem size runs on the sweep kernel K1; two calls
+ * return identical bytes.  Edge residuals are not modelled.
+ * Observability: an offset b is seen because its correction b u changes direction across a frame, and the scale s is told apart
+ * from b by boards seen at different ranges.  Boards in a narrow band of ranges leave s and b nearly collinear with the
+ * translation: clc_information_range_bias then shows a small singular value whose V column lies in the span of e_b, e_s and the
+ * translation; holding s (fixed_mask bit 7) restores full rank.
+ * Rejected before the device is touched, with CLC_ERR_INVALID: a NULL problem or argument (pose7, bias2), a problem with edge
+ * residuals, a pose7 or bias2 entry that is not finite; with CLC_ERR_STATE: a problem attached to a communicator. */
+/* clc_eval at (pose7, b, s): H64, g8 (may be NULL) and *cost (may be NULL). */
+int clc_eval_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], double H64[64], double g8[8], double* cost);
+/* clc_information at (pose7, b, s) (no loss): H64, b8 = -g, chi, the singular values of H (descending) and the matching right
+ * singular vectors as the columns of V64.  Any output may be NULL. */
+int clc_information_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], double H64[64], double b8[8], double* chi,
+                               double singular_values8[8], double V64[64]);
+/* clc_solve_lm on three parameter blocks: the pose (the reference's PoseLocalParameterization), b and s (1-vectors), all in/out.
+ * Ceres' LM over 8 columns, the parameter tolerance on the 9-vector (pose7, b, s), gradient_max_norm = max(|x - Plus(x, -g)|_inf
+ * over the pose, |g_b|, |g_s|).  opt->fixed_mask bits 0-5 as in clc_solve_lm; bit 6 holds b, bit 7 holds s at their start bits.
+ * summary (may be NULL) and trace as clc_solve_lm's; device_ms covers the whole solve.  Also CLC_ERR_INVALID, checked first: a
+ * fixed_mask outside [0, 255), a trace_cap outside [0, 256] or > 0 without trace. */
+int clc_solve_lm_range_bias(clc_problem* p, double pose7[7], double bias2[2], const clc_lm_options* opt, clc_lm_summary* summary,
+                            clc_lm_iteration* trace, int trace_cap);
+/* A new problem on src's device whose points are kappa p of src's (the same frames, planes, poses and loss): every other call
+ * then runs on the corrected points -- trim, quantiles, frame report, select, segments, starts.  Computed on the device from src's
+ * points (nothing is uploaded but the copy's frame offsets and gather plan); two calls give identical points.  Owned by the caller
+ * (clc_problem_destroy).  CLC_ERR_INVALID before any device work: a NULL argument, a bias2 entry that is not finite, 1 + s <= 0,
+ * a problem with edge residuals. */
+int clc_problem_range_correct(const clc_problem* src, const double bias2[2], clc_problem** out);
+
 /* replaces: CamLaserCalClosedSolution(), reference src/LaseCamCalCeres.cpp:112-203.  Tlc16 row-major.
  * AtA81/Atb9 (the 9x9 normal equations) may be NULL. */
 int clc_closed_form(clc_problem* p, double Tlc16[16], int* unobservable, double AtA81[81], double Atb9[9]);
@@ -537,6 +573,9 @@ int clc_bench_poses(clc_problem* p, int64_t n_poses, const double* poses, int n,
 /* The same for one time-offset iteration at (pose7, td): each bracket holds the frames' planes and constants, the segment sweep,
  * the fix-up into 36 sums per frame and the two-level reduction (clc_eval_time_offset without the copy to the host). */
 int clc_bench_time_offset(clc_problem* p, const double pose7[7], double td, int n, int flush_l2, float* ms_each);
+/* The same for one range-bias iteration at (pose7, b, s): each bracket holds the frame constants, the kModeRange sweep, the fix-up
+ * into 45 sums per frame and the two-level reduction (clc_eval_range_bias without the copy to the host). */
+int clc_bench_range_bias(clc_problem* p, const double pose7[7], const double bias2[2], int n, int flush_l2, float* ms_each);
 /* clc_select_frames(p, pose7, desc) with the report computed once and the selection run `n` times on its device rows: ms_each[n]
  * receives the device time of each selection, from its first kernel to the end of its last step (the host polls between step
  * batches included), and *n_selected the picks of the last run. */
